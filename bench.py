@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — mel-frames/sec of the F5TTS.sample() hot path on B200 (BASELINE.json metric).
+"""bench.py — mel-frames/sec of the F5TTS.sample() hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one F5TTS.sample() ODE solve of one batch of synthetic utterances per GPU
@@ -14,7 +14,7 @@ utterance = 937 mel frames (328 ref + 609 gen), 152 text tokens, Euler, steps=32
   e2e        : same metric through the public API a user calls — F5TTS.sample(raw wave on the
                HOST, text) -> waveform on the HOST: H2D of the reference audio + noise, log-mel
                front-end, ODE loop, Vocos vocoder, D2H of the waveform, all inside the timed region
-  roofline   : tcgen05 GEMM family (the dominant kernels): algorithmic FLOPs / summed in-situ duration
+  roofline   : wgmma GEMM family (the dominant kernels): algorithmic FLOPs / summed in-situ duration
                of its launches INSIDE the replayed CUDA graph (per-launch %globaltimer stamps: first
                CTA past the dependency wait -> last CTA exit), so family time <= ms_per_step
   configs    : BASELINE configs 3 (64 x 10 s, midpoint; = config 4 at --gpus 8) and 5 (60 s long-form)
@@ -23,6 +23,10 @@ utterance = 937 mel frames (328 ref + 609 gen), 152 text tokens, Euler, steps=32
                installable here) timed on this box's host cores on a bounded sample of the SAME
                workload
   --impl reference : times only that CPU restatement (rank 0), same metric/config.
+  --dump-outputs DIR : after the timed steps, writes what the last timed step computed as DIR/mel.npy (float32):
+               the mel F5TTS.sample() returns for the headline workload — the conditioning on its masked frames,
+               the sampled frames after them.  Inputs and weights are seeded, so two builds of the project run with
+               the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -42,7 +46,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 SR, HOP = 24000, 256
-TOTAL_SAMPLES, REF_SAMPLES, N_TEXT = 240000, 84000, 152      # SURVEY §8d synthetic "10 s" utterance
+TOTAL_SAMPLES, REF_SAMPLES, N_TEXT = 240000, 84000, 152      # synthetic "10 s" utterance
 
 
 def synth_audio(length: int, seed: int) -> torch.Tensor:
@@ -106,44 +110,14 @@ class ClockSampler:
                 "power_w": statistics.median(pw) if pw else None}
 
 
-def ncu_traffic() -> dict:
-    """DRAM bytes per launch of the dominant (GEMM) kernels from the committed `ncu --set full` captures of this
-    workload (profiles/*_ncu_full.json, see tools/profile.sh): cold (ncu flushes the caches before every replay) and,
-    when captured, warm (--cache-control none: activations L2-resident as inside a step); None if absent."""
-    import glob, re
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "*_ncu_full.json")))
-    if not files:
-        return {"traffic": None}
-
-    def dram(rec):
-        tot = 0.0
-        for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            m = re.match(r"([0-9.,]+)\s*(\w*)", rec.get(k, "0 byte"))
-            tot += float(m.group(1).replace(",", "")) * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(m.group(2), 1)
-        return tot
-    try:
-        d = json.load(open(files[-1]))
-        cold = [dram(r) for k, v in d.items() if k.startswith("gemm") and "warm" not in k for r in v]
-        warm = [dram(r) for k, v in d.items() if k.startswith("gemm") and "warm" in k for r in v]
-        if not cold:
-            return {"traffic": None}
-        out = {"traffic": sum(cold) / len(cold),
-               "traffic_note": f"mean DRAM read+write bytes per launch over the {len(cold)} block-GEMM launches captured in "
-                               f"{os.path.basename(files[-1])} (cold cache under ncu)"}
-        if warm:
-            out["traffic_warm"] = sum(warm) / len(warm)
-        return out
-    except Exception as e:  # pragma: no cover
-        return {"traffic": None, "traffic_note": f"unreadable profile: {e}"}
-
-
 def peaks() -> dict:
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"bf16_tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "hbm_gbs": d.get("hbm_gbs"),
                 "source": "MEASURED_PEAKS.json (bf16_tflops_sustained: kernels timed inside a long step)"}
-    return {"bf16_tflops": 1400.0, "hbm_gbs": 6650.0, "source": "fallback of B200_PROFILING.md (sustained 1.4 PF)"}
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense BF16 989 TFLOP/s, HBM3 3.35 TB/s, 700 W): a ceiling, not a measurement"}
 
 
 # ---------------------------------------------------------------------------------------------
@@ -262,12 +236,13 @@ class Workload:
                             f"{self.n_text} text tokens), {self.method} steps={self.ode_steps} grid points "
                             f"({self.ode_steps - 1} intervals), CFG={self.cfg}, sway=-1",
                 "global_batch": self.batch * world, "frames": self.frames, "parallelism": f"dp{world}",
-                "l2": "no flush: the 0.67 GB of bf16 weights streamed every DiT evaluation exceed the 126 MB L2"}
+                "l2": "no flush: the 0.67 GB of bf16 weights streamed every DiT evaluation exceed the 50 MB L2"}
 
 
 def measure(f5, lib, wl: Workload, rank: int, world: int, dev, steps: int, warmup: int, clocks=None) -> dict:
     """Timed region = `steps` graph replays (inputs resident); then ONE more replay with the in-graph timing slots
-    reset, from which the per-family device times come (same graph, same stream, inside the step)."""
+    reset, from which the per-family device times come (same graph, same stream, inside the step).
+    res["_outputs"]: what the last timed replay computed, as F5TTS.sample() returns it (mel [B, N, 100] fp32)."""
     import ctypes as C
     import torch.distributed as dist
     B, N, NR = wl.batch, wl.frames, wl.ref_frames
@@ -289,6 +264,15 @@ def measure(f5, lib, wl: Workload, rank: int, world: int, dev, steps: int, warmu
     f5.use_cuda_graph = False
     c0 = lib.f5_launch_count()
     out, _ = f5.sample(cond_d, text, N, y0=y0_d, **kw)
+    # what sample() returns, from the plan's ODE state: the conditioning where cond_mask holds, the sampled frames
+    # after it (cfm.py:395-397).  cond_mask covers max(text tokens, reference frames) frames (cfm.py:302): the same
+    # for every utterance here (no -1 padding in `text`); past NR frames the conditioning is zero padding.
+    ref_rows = (torch.arange(N, device=dev) < max(NR, wl.n_text))[None, :, None]
+    cond_full = torch.nn.functional.pad(cond_d, (0, 0, 0, N - NR))
+
+    def returned_mel():
+        return torch.where(ref_rows, cond_full, f5.last_plan.y[:, :N])
+    assert torch.equal(returned_mel(), out), "bench's reconstruction of sample()'s result disagrees with sample()"
     torch.cuda.synchronize()
     launches_per_step = int(lib.f5_launch_count() - c0)
     assert torch.isfinite(out).all().item(), "non-finite output"
@@ -317,6 +301,7 @@ def measure(f5, lib, wl: Workload, rank: int, world: int, dev, steps: int, warmu
         step()
     e1.record()
     barrier()
+    outputs = {"mel": returned_mel()}
     ms = e0.elapsed_time(e1)
     clk = clocks.stop() if clocks is not None else None
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
@@ -347,8 +332,7 @@ def measure(f5, lib, wl: Workload, rank: int, world: int, dev, steps: int, warmu
     gm, at = fam["gemm"], fam["attention"]
     ach = gm["flops"] / (gm["ms"] * 1e-3) / 1e12 if gm["ms"] > 0 else 0.0
     roof = {"bound": "tensor", "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"],
-            **ncu_traffic(),
-            "kernel": "gemm_bf16_tn_kernel + gemm2_bf16_tn_kernel (tcgen05; every GEMM launch of one step)",
+            "kernel": "gemm_bf16_tn_kernel (wgmma; every GEMM launch of one step)",
             "how": "per-launch in-situ duration inside the replayed CUDA graph: min over CTAs of %globaltimer after the "
                    "dependency wait -> max over CTAs at exit, summed over the family; algorithmic 2MNK flops",
             "of": pk["source"], "gemm_ms_per_step": gm["ms"], "gemm_launches_per_step": gm["launches"],
@@ -364,7 +348,25 @@ def measure(f5, lib, wl: Workload, rank: int, world: int, dev, steps: int, warmu
     if clk is not None:
         res["clocks"] = clk
     res["_inputs"] = (cond, text, y0, kw)
+    res["_outputs"] = outputs
     return res
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(outputs: dict, out_dir: str) -> None:
+    """Each array as <out_dir>/<name>.npy in float32; one larger than the 64 MB budget is replaced by a fixed, seeded
+    sample of its elements (<name>_sample.npy, flat)."""
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(len(outputs), 1)
+    for name, t in outputs.items():
+        a = t.detach().float().cpu()
+        if a.numel() * 4 > budget:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.numel(), generator=g)[: budget // 4].sort().values
+            a, name = a.reshape(-1)[idx], name + "_sample"
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy().astype(np.float32))
 
 
 def run_cuda(args, rank: int, world: int, local_rank: int):
@@ -375,7 +377,7 @@ def run_cuda(args, rank: int, world: int, local_rank: int):
 
     if not torch.cuda.is_available():
         # the product path has no CPU fallback: say so instead of measuring something else
-        sys.stderr.write("bench.py: no CUDA device visible; this arm runs libf5b200.so on a B200 only "
+        sys.stderr.write("bench.py: no CUDA device visible; this arm runs libf5b200.so on an H100 only "
                          "(the CPU baseline is `--impl reference`)\n")
         raise SystemExit(3)
     torch.cuda.set_device(local_rank)
@@ -400,7 +402,7 @@ def run_cuda(args, rank: int, world: int, local_rank: int):
     main_wl = Workload("main", B, N, NR, args.method, args.ode_steps, args.cfg)
 
     if args.profile_run:
-        # under ncu: one eager pass of the same step, then the audio front-end and the vocoder (nothing is timed)
+        # under a profiler: one eager pass of the same step, then the audio front-end and the vocoder (nothing is timed)
         g = torch.Generator().manual_seed(100)
         cond = (torch.randn(B, NR, 100, generator=g) * 2.24 - 1.27).clamp(-11.51, 5.0).to(dev)
         text = torch.randint(0, 2545, (B, N_TEXT), generator=g, dtype=torch.int32)
@@ -420,6 +422,9 @@ def run_cuda(args, rank: int, world: int, local_rank: int):
     clocks = ClockSampler(local_rank)
     m = measure(f5, lib, main_wl, rank, world, dev, args.steps, args.warmup, clocks)
     cond, text, y0, kw = m.pop("_inputs")
+    outputs = m.pop("_outputs")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(outputs, args.dump_outputs)
 
     # ---- end to end through the public API with HOST buffers (same batch as the headline) ----
     e2e_steps = max(2, min(args.steps, 10))
@@ -461,7 +466,7 @@ def run_cuda(args, rank: int, world: int, local_rank: int):
                        (Workload("cfg5_long60s", 1, 5625, 499, "euler", 32, 2.0, n_text=N_TEXT * 6), 3)):
             f5._plans.clear(); model._sessions.clear(); torch.cuda.empty_cache()
             r = measure(f5, lib, wl, rank, world, dev, st, 1)
-            r.pop("_inputs")
+            r.pop("_inputs"); r.pop("_outputs")
             subs[wl.name] = r
         # config 4 of BASELINE.json (512 utterances over 8 GPUs = 64 per GPU, weights broadcast once, no per-step
         # collective) is cfg3_b64_midpoint at --gpus 8: its `value` is the whole-job aggregate over all ranks
@@ -481,7 +486,7 @@ def run_cuda(args, rank: int, world: int, local_rank: int):
                 m8.packed.broadcast(src=0)
             r = measure(F5TTS(m8), lib, Workload("b1_fp8", B, N, NR, args.method, args.ode_steps, args.cfg), rank, world, dev,
                         max(3, min(args.steps, 10)), 3)
-            r.pop("_inputs")
+            r.pop("_inputs"); r.pop("_outputs")
             r["dtype"] = "fp8 (e4m3 operands of QKV / out / FF1 / FF2, fp32 accumulate) + bf16 elsewhere"
             r["note"] = "lossy mode: oracle-emulated drift 2.9e-2 per forward vs 3.9e-3 for bf16 (DESIGN.md section 8)"
             subs["b1_fp8"] = r
@@ -529,10 +534,12 @@ def main():
     ap.add_argument("--cfg", type=float, default=2.0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the config-3 / config-5 sub-results")
-    ap.add_argument("--no-fused-adaln", action="store_true", help="A/B: separate LayerNorm+modulate launches (r01 path)")
+    ap.add_argument("--no-fused-adaln", action="store_true", help="A/B: separate LayerNorm+modulate launches")
     ap.add_argument("--fp8", action="store_true", help="FP8 mode (e4m3 QKV / FF1 GEMMs): the lossy analogue of the reference's --q; "
                                                         "NOT the headline (dtype is reported as fp8+bf16)")
-    ap.add_argument("--profile-run", action="store_true", help="one eager step and exit (for ncu)")
+    ap.add_argument("--profile-run", action="store_true", help="one eager step and exit (for a profiler)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))

@@ -1,4 +1,4 @@
-"""f5_tts_mlx_b200 — B200 (sm_100a) implementation of the f5-tts-mlx sampling hot path.
+"""f5_tts_mlx_b200 — H100 (sm_90a) implementation of the f5-tts-mlx sampling hot path.
 
 Same public surface as the reference package for that path (`from f5_tts_mlx import F5TTS`,
 f5_tts_mlx/__init__.py:1): F5TTS (alias CFM), DiT, MelSpec, generate().  Importing this package

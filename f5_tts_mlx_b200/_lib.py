@@ -1,7 +1,7 @@
 """ctypes binding of libf5b200.so (the C ABI declared in include/f5_b200.h).
 
 There is no fallback: if the shared object is missing the import of any compute module raises, and
-if no sm_100 GPU is present every entry point returns F5_ERR_NO_DEVICE which `check()` turns into a
+if no sm_90 GPU is present every entry point returns F5_ERR_NO_DEVICE which `check()` turns into a
 RuntimeError.
 """
 from __future__ import annotations
@@ -30,7 +30,7 @@ def load() -> C.CDLL:
         if not _LIB_PATH.exists():
             raise F5Error(
                 f"{_LIB_PATH} is missing: build it with `python -m f5_tts_mlx_b200.build` "
-                "(nvcc, sm_100a). This package has no CPU / PyTorch fallback."
+                "(nvcc, sm_90a). This package has no CPU / PyTorch fallback."
             )
         _lib = C.CDLL(str(_LIB_PATH))
         _lib.f5_last_error.restype = C.c_char_p

@@ -1,7 +1,7 @@
 """MelSpec / log_mel_spectrogram — host-side mirror of f5_tts_mlx/audio.py:162-230.
 
 The arithmetic (zero-padded centred framing, periodic-Hann 1024-point real FFT, magnitude, HTK mel
-filterbank, log(max(., 1e-5))) runs in the sm_100a kernel behind `f5_mel_forward`; this module only
+filterbank, log(max(., 1e-5))) runs in the sm_90a kernel behind `f5_mel_forward`; this module only
 builds the two constant tables (window, filterbank) and marshals pointers.
 """
 from __future__ import annotations

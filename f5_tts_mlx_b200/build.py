@@ -1,4 +1,4 @@
-"""In-tree build of libf5b200.so (CUDA, sm_100a only) with plain nvcc.
+"""In-tree build of libf5b200.so (CUDA, sm_90a only) with plain nvcc.
 
 The shared object is written next to this file (f5_tts_mlx_b200/libf5b200.so) so that it travels
 with the source tree; it is git-ignored.  Rebuilds only when a source is newer than the library.
@@ -18,7 +18,7 @@ LIB_PATH = PKG_DIR / "libf5b200.so"
 OBJ_DIR = PKG_DIR / "build"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xptxas=-v",
     "-Xcompiler", "-fPIC",

@@ -3,7 +3,7 @@
 `sample()` keeps the reference's signature, defaults, return value `(out, trajectory)` and error
 behaviour.  Host code here is bookkeeping only (the mask/duration prologue of cfm.py:279-336 on a
 handful of integers, buffer management, CUDA-graph capture); every tensor operation of the hot
-path is an sm_100a kernel in libf5b200 reached through the C ABI (f5_dit_precompute,
+path is an sm_90a kernel in libf5b200 reached through the C ABI (f5_dit_precompute,
 f5_ode_sample, f5_mel_forward, f5_vocos_decode).
 """
 from __future__ import annotations

@@ -1,12 +1,10 @@
-// Host launcher + C-ABI entry for the tcgen05 flash-attention forward (attention2_sm100.cuh).
-#include <stdlib.h>
-
-#include "attention2_sm100.cuh"
+// Host launcher + C-ABI entry for the wgmma flash-attention forward (attention_sm90.cuh).
+#include "attention_sm90.cuh"
 #include "host_common.h"
 
-static unsigned long long* g_attn_ts = nullptr;
+// The attention kernel records no per-tile timeline; the entry point stays for ABI compatibility.
 extern "C" int f5_debug_attention_ts(void* base) {
-  g_attn_ts = reinterpret_cast<unsigned long long*>(base);
+  (void)base;
   return 0;
 }
 
@@ -44,17 +42,6 @@ static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
   p.kv_len = kv_len;
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.ldo = (int)ld_out;
-  p.handoff = 1;
-  // F5_ATTN_HANDOFF: 2 (default) a softmax group is released when the other is half way through its exponentials,
-  // 1 strict alternation, 0 off.  (The smem-P variant and the polynomial-exp2 variants of round 1 — measured neutral or
-  // slower — are no longer instantiated; the template parameters document them.)
-  static int handoff = -1;
-  if (handoff < 0) {
-    const char* ho = getenv("F5_ATTN_HANDOFF");
-    handoff = (ho && ho[0] >= '0' && ho[0] <= '2') ? ho[0] - '0' : 2;
-  }
-  p.handoff = handoff;
-  p.ts = g_attn_ts;
   p.out_fp8 = out_fp8;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfScope ps(PROF_ATTN, 4.0 * batch * heads * (double)frames * frames * 64.0,
@@ -66,8 +53,8 @@ static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
     F5_CHECK_CUDA(cudaGetLastError());
     return 0;
   };
-  const dim3 grid256(cdiv(frames, 256), heads, batch);
+  const dim3 grid(cdiv(frames, 128), heads, batch);
   static SmemAttrOnce o4, o8;
-  if (out_fp8) return launch(attn2_fwd_kernel<true, 0, true>, o8, grid256, 384, Attn2Smem::kTotal);
-  return launch(attn2_fwd_kernel<true, 0, false>, o4, grid256, 384, Attn2Smem::kTotal);
+  if (out_fp8) return launch(attn_fwd_kernel<true>, o8, grid, 384, AttnSmem::kTotal);
+  return launch(attn_fwd_kernel<false>, o4, grid, 384, AttnSmem::kTotal);
 }

@@ -1,5 +1,5 @@
 // Log-mel front-end (audio.py:115-210) and the Vocos back-end (vocos_mlx.Vocos.decode, call site
-// cfm.py:399-400) for sm_100a.  FFTs are warp-level (fft.cuh): one warp = one frame.
+// cfm.py:399-400) for sm_90a.  FFTs are warp-level (fft.cuh): one warp = one frame.
 #include <string.h>
 
 #include "fft.cuh"

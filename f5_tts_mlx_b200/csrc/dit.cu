@@ -1,4 +1,4 @@
-// DiT forward and the ODE loop of F5TTS.sample as a stream-ordered sequence of the sm_100a kernels
+// DiT forward and the ODE loop of F5TTS.sample as a stream-ordered sequence of the sm_90a kernels
 // in this directory (C-ABI: f5_dit_precompute / f5_dit_forward / f5_ode_sample).
 //
 // What the reference recomputes on every forward but depends only on (text, cond, t) is hoisted:

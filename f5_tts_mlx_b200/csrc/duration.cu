@@ -1,5 +1,5 @@
 // DurationPredictor forward (duration.py:97-253, inference branch) as a stream-ordered sequence of
-// the same sm_100a kernels the DiT uses: TextEmbedding (mask_padding=False, 2 ConvNeXtV2 blocks),
+// the same sm_90a kernels the DiT uses: TextEmbedding (mask_padding=False, 2 ConvNeXtV2 blocks),
 // DurationInputEmbedding (Linear on [mel | text] + ConvPositionEmbedding), `depth` DurationBlocks
 // (plain LayerNorm -> attention (no mask, duration.py:245) -> residual -> LayerNorm -> FF -> residual),
 // RMSNorm + masked mean + Linear(dim->1) + Softplus.  Runs once per sample() when duration=None

@@ -1,4 +1,4 @@
-// HBM-bound kernels of the DiT path (sm_100a).  All are coalesced / 128-bit vectorised, one warp
+// HBM-bound kernels of the DiT path (sm_90a).  All are coalesced / 128-bit vectorised, one warp
 // per frame row where a row reduction is needed, fp32 arithmetic, bf16 only as the tensor-core
 // operand they hand to the next GEMM.
 #pragma once

@@ -1,4 +1,4 @@
-// Warp-level 512-point complex FFT (sm_100a): 16 points per lane in registers (radix-2 DIF,
+// Warp-level 512-point complex FFT (sm_90a): 16 points per lane in registers (radix-2 DIF,
 // fully unrolled, compile-time twiddles) x 32 lanes via shuffle butterflies.  A 1024-point real
 // FFT / inverse real FFT is one such transform plus an O(N) split step.
 //

@@ -1,15 +1,8 @@
-// Host launcher + C-ABI entry for the tcgen05 GEMM (see gemm_sm100.cuh and include/f5_b200.h).
+// Host launcher + C-ABI entry for the wgmma GEMM (see gemm_sm90.cuh and include/f5_b200.h).
 #include <stdlib.h>
 
-#include "gemm_sm100.cuh"
-#include "gemm2_sm100.cuh"
+#include "gemm_sm90.cuh"
 #include "host_common.h"
-
-// operand-ring depth of the one-CTA-per-SM kernel: the main loop is bound by bytes in flight / TMA latency (r02: the
-// same 400 clk per k-block with 8 or 120 CTAs running), so the ring takes all the shared memory there is
-#ifndef F5_ONEWAVE_STAGES
-#define F5_ONEWAVE_STAGES 6
-#endif
 
 namespace f5 {
 
@@ -27,7 +20,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
                stream);
   GemmParams q = p;
   q.prof = ps.slot;
-  F5_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GemmEpi<BN, kStages, ROPE, RESID>::kThreads), S::kTotal, stream, ta, tb, to, to2, q));
+  F5_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GemmEpi<BN>::kThreads), S::kTotal, stream, ta, tb, to, to2, q));
   F5_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -37,8 +30,8 @@ static int dispatch_epi(int act, bool out_bf16, bool rope, const CUtensorMap& ta
                         const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2, const GemmParams& p,
                         dim3 grid, cudaStream_t stream) {
   const bool fp8 = p.ab8 || p.out_fp8 || p.out2_fp8;     // e4m3 features: separate instantiations (what the FP8 mode of the DiT uses)
-  // residual-free GELU epilogue of the two-CTAs-per-SM variant (FF1 at batch 1): two epilogue groups (gemm_sm100.cuh)
-  if (BN == 128 && kStages == 3 && p.resid == nullptr && act == ACT_GELU_TANH && out_bf16 && !rope) {
+  // residual-free GELU epilogue (FF1): no residual tiles in the epilogue's registers
+  if (p.resid == nullptr && act == ACT_GELU_TANH && out_bf16 && !rope) {
     if (fp8) return launch_gemm<BN, kStages, ACT_GELU_TANH, true, false, true, false>(ta, tb, to, to2, p, grid, stream);
     return launch_gemm<BN, kStages, ACT_GELU_TANH, true, false, false, false>(ta, tb, to, to2, p, grid, stream);
   }
@@ -53,55 +46,6 @@ static int dispatch_epi(int act, bool out_bf16, bool rope, const CUtensorMap& ta
   if (fp8) return set_error(F5_ERR_INVALID, "f5_gemm_bf16: FP8 features are not built for epilogue act=%d out_bf16=%d rope=%d", act, (int)out_bf16, (int)rope);
 #define F5_CASE(A, O, R) \
   if (act == A && out_bf16 == O && rope == R) return launch_gemm<BN, kStages, A, O, R, false>(ta, tb, to, to2, p, grid, stream);
-  F5_CASE(ACT_NONE, true, true)
-  F5_CASE(ACT_NONE, true, false)
-  F5_CASE(ACT_NONE, false, false)
-  F5_CASE(ACT_GELU_TANH, true, false)
-  F5_CASE(ACT_GELU_ERF, true, false)
-  F5_CASE(ACT_MISH, true, false)
-  F5_CASE(ACT_MISH, false, false)
-#undef F5_CASE
-  return set_error(F5_ERR_INVALID, "f5_gemm_bf16: unsupported epilogue act=%d out_bf16=%d rope=%d",
-                   act, (int)out_bf16, (int)rope);
-}
-
-template <int BN, int kStages, int ACT, bool OUT_BF16, bool ROPE, bool FP8>
-static int launch_gemm2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2,
-                        const GemmParams& p, int n_tiles, int total_tiles, cudaStream_t stream) {
-  using S = Gemm2Smem<BN, kStages, Gemm2Lno<BN, OUT_BF16>::value>;
-  auto kern = gemm2_bf16_tn_kernel<BN, kStages, ACT, OUT_BF16, ROPE, FP8>;
-  static SmemAttrOnce once;
-  F5_CHECK_CUDA(ensure_dyn_smem(once, kern, S::kTotal));
-  const int num_pairs = sm_count() / 2;
-  const int clusters = total_tiles < num_pairs ? total_tiles : num_pairs;
-  const double taps = p.conv_taps;
-  ProfScope ps(PROF_GEMM, 2.0 * p.M * (double)p.N * (double)p.k_per_tap * taps,
-               2.0 * ((double)p.M * p.k_per_tap + (double)p.N * p.k_per_tap * taps) +
-                   (double)p.M * p.N * (OUT_BF16 ? 2.0 : 4.0),
-               stream);
-  GemmParams q = p;
-  q.prof = ps.slot;
-  F5_CHECK_CUDA(launch_kernel(kern, dim3(2 * clusters), dim3(384), S::kTotal, stream, ta, tb, to, to2, q, n_tiles, total_tiles));
-  F5_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int BN, int kStages>
-static int dispatch_epi2(int act, bool out_bf16, bool rope, const CUtensorMap& ta,
-                         const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2, const GemmParams& p,
-                         int n_tiles, int total_tiles, cudaStream_t stream) {
-  const bool fp8 = p.ab8 || p.out_fp8 || p.out2_fp8;
-#define F5_CASE8(A, O, R) \
-  if (fp8 && act == A && out_bf16 == O && rope == R) return launch_gemm2<BN, kStages, A, O, R, true>(ta, tb, to, to2, p, n_tiles, total_tiles, stream);
-  F5_CASE8(ACT_NONE, true, true)
-  F5_CASE8(ACT_NONE, true, false)
-  F5_CASE8(ACT_NONE, false, false)
-  F5_CASE8(ACT_GELU_TANH, true, false)
-  F5_CASE8(ACT_MISH, false, false)
-#undef F5_CASE8
-  if (fp8) return set_error(F5_ERR_INVALID, "f5_gemm_bf16: FP8 features are not built for epilogue act=%d out_bf16=%d rope=%d", act, (int)out_bf16, (int)rope);
-#define F5_CASE(A, O, R) \
-  if (act == A && out_bf16 == O && rope == R) return launch_gemm2<BN, kStages, A, O, R, false>(ta, tb, to, to2, p, n_tiles, total_tiles, stream);
   F5_CASE(ACT_NONE, true, true)
   F5_CASE(ACT_NONE, true, false)
   F5_CASE(ACT_NONE, false, false)
@@ -190,104 +134,19 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
     }
   }
 
-  int variant = a->variant;
-  {
-    static int forced = -1;   // debugging aid: F5_GEMM_VARIANT=1|2 overrides the automatic choice
-    if (forced < 0) {
-      const char* v = getenv("F5_GEMM_VARIANT");
-      forced = v ? atoi(v) : 0;
-    }
-    if (forced == 1 || forced == 2) variant = forced;
-  }
-  if (a->conv_grouped) variant = 1;            // grouped conv: 64-wide column blocks, single-CTA kernel
-  if (variant == 0) {
-    // measured on B200 (tests/gpu_checks/check_gemm2.py): the persistent CTA-pair kernel with 256-wide
-    // tiles wins whenever there are enough 256x256 tiles to fill the 74 SM pairs (large M: 1.2-1.35
-    // PFLOP/s vs 0.85-1.0), and for wide outputs (N >= 3072) even at M ~ 2k; the single-CTA kernel
-    // with 128x128 tiles spreads small problems over more SMs.
-    const long long pair_tiles = (long long)cdiv(a->m, 256) * cdiv(a->n, 256);
-    const int sms = sm_count();
-    variant = (a->n >= 128 && (pair_tiles >= sms || (pair_tiles >= sms / 2 && a->n >= 3072))) ? 2 : 1;
-  }
-  // pair kernel: a second output (out2 / fused-LN producer mode) with 256-wide tiles only
-  if (variant == 2 && a->out2_bf16 && a->tile_n != 0 && a->tile_n != 256) variant = 1;
-  if (variant == 2 && a->out2_bf16 && !(a->n % 256 == 0 || a->n >= 1024)) variant = 1;
-  if (variant == 2) {
-    int bn2 = a->tile_n;
-    if (bn2 == 0) bn2 = (a->n % 256 == 0 || a->n >= 1024) ? 256 : 128;
-    // wide outputs on few row tiles (QKV at batch 1: 8 x 12 tiles of 256 columns on 74 SM pairs = two rounds, the
-    // second 30 % full): narrower tiles — 8 x 16 of 192 or 8 x 24 of 128 columns — only when they remove a mostly
-    // empty round; at equal cost the narrower tile wins (r02, same box: 128-wide 51.8 vs 192-wide 53.0 ms per step —
-    // its exposed last epilogue is two chunks per group instead of three, and three rounds overlap more of them)
-    if (a->tile_n == 0 && bn2 == 256 && !a->out2_bf16) {
-      const int pairs = sm_count() / 2, mt = cdiv(a->m, 256);
-      const double c256 = (double)cdiv(mt * cdiv(a->n, 256), pairs) * 256;
-      double best = c256;
-      if (a->n % 192 == 0) {
-        const double c192 = (double)cdiv(mt * cdiv(a->n, 192), pairs) * 192;
-        if (c192 < 0.85 * c256) { bn2 = 192; best = c192; }
-      }
-      if (a->n % 128 == 0) {
-        const double c128 = (double)cdiv(mt * cdiv(a->n, 128), pairs) * 128;
-        if (c128 < 0.85 * c256 && c128 <= best) bn2 = 128;
-      }
-    }
-    F5_REQUIRE(bn2 == 128 || bn2 == 192 || bn2 == 256, "f5_gemm_bf16: CTA-pair tile_n must be 128, 192 or 256");
-    GemmParams p2;
-    p2.M = a->m; p2.N = a->n; p2.K = a->k;
-    p2.rows_per_batch = rpb;
-    p2.tiles_per_batch = batched ? cdiv(rpb, 256) : 0;
-    p2.num_batches = nb;
-    p2.conv_taps = taps; p2.conv_pad = a->conv_pad; p2.k_per_tap = a->k; p2.conv_grouped = 0;
-    p2.bias = a->bias; p2.out = a->out; p2.ldo = (int)a->ldo;
-    p2.resid = a->resid; p2.ldr = (int)a->ldr;
-    p2.gate = a->gate; p2.gate_ld = (int)a->gate_ld;
-    p2.row_len = a->row_len;
-    p2.rope = reinterpret_cast<const float2*>(a->rope);
-    p2.rope_cols = a->rope_cols; p2.q_scale = a->q_scale; p2.q_cols = a->q_cols;
-    p2.out2 = reinterpret_cast<__nv_bfloat16*>(a->out2_bf16); p2.ldo2 = (int)a->ldo2;
-    p2.ts = reinterpret_cast<unsigned long long*>(a->debug_ts);
-    p2.w_static = a->w_static;
-    p2.pf_ptr = reinterpret_cast<const char*>(a->prefetch); p2.pf_bytes = a->prefetch_bytes;
-    p2.ln_scale = a->ln_scale; p2.ln_stats = reinterpret_cast<float2*>(a->ln_stats);
-    p2.ln_in_stats = reinterpret_cast<const float2*>(a->ln_in_stats); p2.ln_in_units = a->k / 64;
-    p2.ln_tab = a->ln_tab; p2.ln_tab_ld = a->ln_tab_ld;
-    p2.ab8 = ab8 ? 1 : 0; p2.acc_scale = ab8 ? a->acc_scale : 1.f; p2.out2_fp8 = a->out2_fp8; p2.out_fp8 = a->out_fp8;
-    if (a->out2_bf16) F5_REQUIRE(a->ldo2 % 8 == 0 && a->n % 8 == 0, "f5_gemm_bf16: out2 alignment");
-    CUtensorMap ta2, tb2;
-    {
-      uint64_t dims[3] = {(uint64_t)a->k, (uint64_t)(batched ? rpb : a->m), (uint64_t)(batched ? nb : 1)};
-      uint64_t str[2] = {(uint64_t)a->lda * esz, (uint64_t)a->lda * esz * (uint64_t)rpb};
-      uint32_t box[3] = {kbox, 128, 1};
-      if (int e = (ab8 ? make_tmap_u8 : make_tmap_bf16)(&ta2, a->a, 3, dims, str, box)) return e;
-    }
-    {
-      const int kpad = cdiv(a->k, 64) * 64;
-      uint64_t dims[2] = {(uint64_t)(taps == 1 ? a->k : taps * kpad), (uint64_t)a->n};
-      uint64_t str[1] = {(uint64_t)a->ldw * esz};
-      uint32_t box[2] = {kbox, (uint32_t)(bn2 / 2)};
-      if (int e = (ab8 ? make_tmap_u8 : make_tmap_bf16)(&tb2, a->w, 2, dims, str, box)) return e;
-    }
-    const int n_tiles = cdiv(a->n, bn2);
-    const int m_tiles = batched ? nb * cdiv(rpb, 256) : cdiv(a->m, 256);
-    cudaStream_t stream2 = reinterpret_cast<cudaStream_t>(stream_);
-    const bool rope2 = a->rope != nullptr;
-    if (bn2 == 192)
-      return dispatch_epi2<192, 5>(a->act, a->out_bf16 != 0, rope2, ta2, tb2, to, to2, p2, n_tiles, n_tiles * m_tiles, stream2);
-    if (bn2 == 256)
-      return dispatch_epi2<256, 4>(a->act, a->out_bf16 != 0, rope2, ta2, tb2, to, to2, p2, n_tiles, n_tiles * m_tiles, stream2);
-    return dispatch_epi2<128, 6>(a->act, a->out_bf16 != 0, rope2, ta2, tb2, to, to2, p2, n_tiles, n_tiles * m_tiles, stream2);
-  }
-
-  int bn = a->tile_n;
+  // tile width: 64 or 128 columns.  `variant` selects nothing on sm_90 (there is one kernel family); wider tile
+  // requests (192, 256) get the widest tile there is.
+  F5_REQUIRE(a->variant >= 0 && a->variant <= 2, "f5_gemm_bf16: variant must be 0, 1 or 2");
+  F5_REQUIRE(a->tile_n == 0 || a->tile_n == 64 || a->tile_n == 128 || a->tile_n == 192 || a->tile_n == 256,
+             "f5_gemm_bf16: tile_n must be 0, 64, 128, 192 or 256");
+  int bn = a->tile_n > 128 ? 128 : a->tile_n;
   if (a->conv_grouped) bn = 64;
   if (bn == 0) {
-    // fill the 148 SMs: prefer 128-wide tiles unless that leaves most SMs idle
+    // fill the SMs: prefer 128-wide tiles unless that leaves most SMs idle
     const int mt = batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128);
     bn = (mt * cdiv(a->n, 128) >= (sm_count() * 13) / 16 || a->n <= 64) ? 128 : 64;
     if (a->n <= 64) bn = 64;
   }
-  F5_REQUIRE(bn == 64 || bn == 128, "f5_gemm_bf16: tile_n must be 64 or 128");
 
   GemmParams p;
   p.M = a->m; p.N = a->n; p.K = a->k;
@@ -338,10 +197,6 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   dim3 grid(cdiv(a->n, bn), batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128), 1);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const bool rope = a->rope != nullptr;
-  // grids that fit in one wave leave one CTA per SM anyway: spend the whole smem on a 6-stage ring
-  // (192 KB in flight per SM instead of 96 KB) to cover the L2/HBM latency of the operand stream
-  if (bn == 128 && (long long)grid.x * grid.y <= sm_count())
-    return dispatch_epi<128, F5_ONEWAVE_STAGES>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
-  if (bn == 128) return dispatch_epi<128, 3>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
-  return dispatch_epi<64, 4>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
+  if (bn == 128) return dispatch_epi<128, 4>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
+  return dispatch_epi<64, 6>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
 }

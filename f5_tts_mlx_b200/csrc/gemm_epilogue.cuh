@@ -1,15 +1,11 @@
-// Fused GEMM epilogue shared by the single-CTA (gemm_sm100.cuh) and the 2-CTA persistent
-// (gemm2_sm100.cuh) kernels: one thread owns one output row and 32 consecutive accumulator columns.
+// Fused GEMM epilogue of the wgmma GEMM (gemm_sm90.cuh): one thread owns one output row and 32 consecutive
+// accumulator columns, read from the fp32 accumulator tile the consumer warpgroups left in shared memory.
 #pragma once
 #include "ptx.cuh"
 
 namespace f5 {
 
 enum GemmAct { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF = 2, ACT_MISH = 3 };
-
-#ifndef F5_EPI_WAIT_MODE
-#define F5_EPI_WAIT_MODE 0
-#endif
 
 struct GemmParams {
   int M, N, K;             // logical problem (flat mode: M rows; batched mode: see below)
@@ -54,7 +50,7 @@ struct GemmParams {
   const float* ln_tab;        // 4 rows of ln_tab_ld floats: c1_hi, c1_lo, c2_hi, c2_lo (bf16-split operand rows of
   long long ln_tab_ld;        //   the table GEMM), already offset to this GEMM's column 0
   // ---- FP8 mode of the block GEMMs (DESIGN.md section 8) ----
-  int ab8;                 // A and W are e4m3 bytes: 128-element k-blocks, kind::f8f6f4 MMAs
+  int ab8;                 // A and W are e4m3 bytes: 128-element k-blocks, e4m3 wgmma
   float acc_scale;         // multiplies the accumulator (the weight tensor's quantisation scale); 1 otherwise
   int out2_fp8;            // the second output is e4m3 (1 byte per element) instead of bf16
   int out_fp8;             // the primary output is e4m3 (bf16-output instantiations only): 32-byte rows per chunk
@@ -62,8 +58,7 @@ struct GemmParams {
 
 // Each CTA touches its 1/num_ctas slice of [pf_ptr, pf_ptr + pf_bytes) with L2 prefetches (one warp,
 // 128 B per lane per iteration).  At batch 1 the 0.67 GB of weights stream from HBM once per DiT
-// evaluation and every GEMM used to start cold (3-stage TMA ring vs ~1 us HBM latency per k-block);
-// HBM has >20x the bandwidth this needs, so the next GEMMs' weights are fetched ahead of time.
+// evaluation and every GEMM would otherwise start cold, so the next GEMMs' weights are fetched ahead of time.
 __device__ __forceinline__ void prefetch_slice_l2(const GemmParams& p, int cta, int num_ctas, int lane) {
   if (p.pf_ptr == nullptr) return;
   const long long per = (((p.pf_bytes + num_ctas - 1) / num_ctas) + 127) & ~127LL;
@@ -82,9 +77,8 @@ __device__ __forceinline__ void ts_mark(const GemmParams& p, int cta, int slot) 
 }
 
 // ---------------------------------------------------------------------------------------------
-// Epilogue, organised for memory-level parallelism.  In-situ timelines of the B=1 step showed the
-// first version (load bias -> use -> load gate -> use -> load residual -> use, per 32-column chunk,
-// libm tanhf) spending ~10 us per GEMM in the epilogue against a 6 us main loop.  Now:
+// Epilogue, organised for memory-level parallelism (a load -> use chain per operand and chunk leaves the
+// epilogue latency-bound):
 //   * bias and gate of the tile's columns are staged in shared memory once (epi_stage_cols);
 //   * the RoPE cos/sin of the thread's row (32 pairs = one head) are loaded into registers BEFORE the
 //     accumulator is awaited (epi_load_rope), as is the residual of the first chunk; the residual of
@@ -164,21 +158,6 @@ __device__ __forceinline__ void epi_load_rope(const GemmParams& p, int pos, floa
   }
 }
 
-// only the (cos, sin) pairs of one 32-column half of a head: cs[16 half .. 16 half + 16)
-template <bool ROPE>
-__device__ __forceinline__ void epi_load_rope_half(const GemmParams& p, int pos, float2 (&cs)[ROPE ? 32 : 1], int half) {
-  if (ROPE) {
-    const float4* rp = reinterpret_cast<const float4*>(p.rope + (size_t)pos * 32 + half * 16);
-    if (half == 0) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { const float4 v = rp[j]; cs[2 * j] = make_float2(v.x, v.y); cs[2 * j + 1] = make_float2(v.z, v.w); }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { const float4 v = rp[j]; cs[16 + 2 * j] = make_float2(v.x, v.y); cs[17 + 2 * j] = make_float2(v.z, v.w); }
-    }
-  }
-}
-
 __device__ __forceinline__ void epi_load_resid(const GemmParams& p, int row, int col0, bool row_ok,
                                                float4 (&r)[8]) {
   if (p.resid != nullptr && row_ok && col0 < p.N) {
@@ -192,9 +171,7 @@ __device__ __forceinline__ void epi_load_resid(const GemmParams& p, int row, int
 }
 
 // Stores: a thread owns a ROW, so direct 16-byte stores would land in 32 different rows per warp instruction
-// (half-sector writes 4 KB apart — measured 5-6 us per 128x128 fp32 tile in situ), and even when re-read from a
-// staging buffer and stored cooperatively the LSU path moved only ~20 B/clk per SM (r02 in-situ: 64 KB per CTA in
-// ~2.5 us, +1.5 us for 32 KB more).  So every chunk (128 rows x 32 columns) is written to shared memory in the
+// (half-sector writes 4 KB apart).  So every chunk (128 rows x 32 columns) is written to shared memory in the
 // layout of a swizzled TMA box (fp32: 128-byte rows, SWIZZLE_128B; bf16: 64-byte rows, SWIZZLE_64B — the XOR patterns
 // below are exactly those) and ONE thread hands it to the TMA unit (cp.async.bulk.tensor store), which also clips
 // rows / columns outside the matrix.  Two staging buffers alternate; per chunk one named barrier (128 threads).
@@ -205,8 +182,6 @@ struct EpiStage {
   int et;                  // epilogue thread 0..127 of the group; thread 0 issues the TMA stores
   int r;                   // this thread's row inside the tile
   int bar_id;              // named barrier of this group of 4 epilogue warps (1 + group)
-  int probe_cta;           // debug (F5_EPI_PROBE builds): linear CTA id for sub-step stamps
-  unsigned long long* probe;   // debug: this CTA's timeline row (GemmParams::ts + 10 * cta) or nullptr
   const CUtensorMap* map_out;   // (cols, rows per utterance, utterances) of `out` / `out2`
   const CUtensorMap* map_out2;
   int c1, c2;              // tensor-map coordinates of tile row 0: row inside the utterance, utterance
@@ -215,21 +190,6 @@ struct EpiStage {
   float mu_r, rstd;        // fused-LN consumer mode: this thread's row statistics ((0, 1) otherwise)
 };
 
-// Sub-step stamps of the first epilogue group's thread 0 (debug builds -DF5_EPI_PROBE=1..5, slots 3 and 4 of the
-// per-CTA timeline, which the producer leaves free in those builds): which part of a chunk's latency chain costs what.
-#ifdef F5_EPI_PROBE
-#define F5_EPI_MARK(level, cond, slot)                                                              \
-  do {                                                                                              \
-    if (F5_EPI_PROBE == (level) && st.probe != nullptr && st.et == 0 && st.bar_id == 1 && (cond)) { \
-      unsigned long long t_;                                                                        \
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));                                        \
-      st.probe[slot] = t_;                                                                          \
-    }                                                                                               \
-  } while (0)
-#else
-#define F5_EPI_MARK(level, cond, slot) do { } while (0)
-#endif
-
 // `w2`: the chunk's second output (bf16, 4 x uint4 per row) or nullptr
 // `w2_fp8`: the second output is e4m3 — 32-byte rows, SWIZZLE_32B (16-byte chunk index ^ bit 7 of the row offset)
 template <bool OUT_BF16>
@@ -237,20 +197,11 @@ __device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiSta
                                               const uint4* w2 = nullptr, bool w2_fp8 = false) {
   uint8_t* buf = st.buf + par * 16384;
   uint8_t* buf2 = st.buf2 + par * st.buf2_par;
-  F5_EPI_MARK(2, par == 0, 3);     // chunk 0: math done
-  F5_EPI_MARK(4, par == 1, 4);     // chunk 1: math done
-#if F5_EPI_WAIT_MODE == 1
-  // two barriers per chunk: the buffer about to be rewritten was the source of the store before the previous one;
-  // the previous chunk's store may still be in flight while this chunk is computed and staged
-  if (st.et == 0) { if (w2 != nullptr && st.buf2_par == 0) tma_store_wait_read<0>(); else tma_store_wait_read<1>(); }
-  asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
-#else
   if (w2 != nullptr && st.buf2_par == 0) {
     // one staging buffer for the second output: the previous chunk's store must have read it
     if (st.et == 0) tma_store_wait_read<0>();
     asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
   }
-#endif
   if (OUT_BF16 && st.out_fp8) {
     uint8_t* mine = buf + st.r * 32;           // e4m3: 32-byte rows, SWIZZLE_32B
     const int sw = (st.r >> 2) & 1;
@@ -290,23 +241,15 @@ __device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiSta
     }
   }
   fence_proxy_async_smem();                           // generic-proxy writes -> visible to the TMA unit
-  F5_EPI_MARK(2, par == 0, 4);     // chunk 0: staged + fenced
-#if F5_EPI_WAIT_MODE != 1
   // the OTHER staging buffer is rewritten by the next chunk: every store issued so far must have read its source
   // (the previous chunk's store was issued a whole chunk of work ago)
   if (st.et == 0) tma_store_wait_read<0>();
-#endif
-  F5_EPI_MARK(3, par == 0, 3);     // chunk 0: previous store's reads done (none for chunk 0)
-  F5_EPI_MARK(5, par == 1, 3);     // chunk 1: chunk 0's store has read its staging buffer
   asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
-  F5_EPI_MARK(3, par == 0, 4);     // chunk 0: group barrier passed
   if (st.et == 0) {
     tma_store_3d(st.map_out, buf, col0, st.c1, st.c2);
     if (w2 != nullptr) tma_store_3d(st.map_out2, buf2, col0, st.c1, st.c2);
     tma_store_commit();
   }
-  F5_EPI_MARK(4, par == 0, 3);     // chunk 0: stores issued
-  F5_EPI_MARK(5, par == 1, 4);     // chunk 1: stores issued (epi_end - this = the final wait for the store's reads)
 }
 
 // HALF: which 32-column half of a 64-column head this chunk is (static RoPE register indexing)
@@ -436,94 +379,42 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
   epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0);   // all 128 threads of the group take part (barrier inside)
 }
 
-// Drains one accumulator tile of BN columns: TMEM base `tmem_acc` (lane group already applied).
-// (cc0, cc_step): this group of 4 warps takes the 64-column units cc0, cc0 + cc_step, ... (two groups
-// interleave units in the CTA-pair kernel); `res0` holds the residual of unit cc0's first 32 columns.
+// 32 consecutive fp32 accumulator columns of this thread's row (shared memory, 16-byte aligned)
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&acc)[32]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float4 v = *reinterpret_cast<const float4*>(src + 4 * j);
+    acc[4 * j] = __float_as_uint(v.x); acc[4 * j + 1] = __float_as_uint(v.y);
+    acc[4 * j + 2] = __float_as_uint(v.z); acc[4 * j + 3] = __float_as_uint(v.w);
+  }
+}
+
+// Drains one accumulator tile of BN columns: `acc_row` = this thread's row of the shared-memory accumulator tile,
+// already offset to the group's first column.  `res0` holds the residual of the first 32 columns.
 template <int BN, int ACT, bool OUT_BF16, bool ROPE>
-__device__ __forceinline__ void epi_drain_tile(uint32_t tmem_acc, const float* bias_s,
+__device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float* bias_s,
                                                const float* gate_s, const float* aux_s, const float2 (&cs)[ROPE ? 32 : 1],
                                                float4 (&res0)[8], const GemmParams& p, int n0, int row,
-                                               int b_idx, bool row_ok, bool row_valid,
-                                               EpiStage& st, int cc0 = 0, int cc_step = 1) {
+                                               int b_idx, bool row_ok, bool row_valid, EpiStage& st) {
   float4 res1[8];
   float2 unit_acc = make_float2(0.f, 0.f);
   st.par_base = 0;
 #pragma unroll 1
-  for (int cc = cc0; cc < BN / 64; cc += cc_step) {
+  for (int cc = 0; cc < BN / 64; ++cc) {
     const int colA = n0 + cc * 64, colB = colA + 32;
     uint32_t acc[32];
     // chunk A (first half of the head): request chunk B's residual, then drain A
     epi_load_resid(p, row, colB, row_ok, res1);
-    tmem_ld32(tmem_acc + cc * 64, acc);
-    tmem_wait_ld();
+    acc_ld32(acc_row + cc * 64, acc);
     if (colA < p.N)   // uniform per CTA
       epi_apply<ACT, OUT_BF16, ROPE, 0>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
                                         b_idx, row_ok, row_valid, st, unit_acc);
     // chunk B: request the next unit's first residual, then drain B
-    if (cc + cc_step < BN / 64) epi_load_resid(p, row, colA + 64 * cc_step, row_ok, res0);
-    tmem_ld32(tmem_acc + cc * 64 + 32, acc);
-    tmem_wait_ld();
+    if (cc + 1 < BN / 64) epi_load_resid(p, row, colA + 64, row_ok, res0);
+    acc_ld32(acc_row + cc * 64 + 32, acc);
     if (colB < p.N)
       epi_apply<ACT, OUT_BF16, ROPE, 1>(acc, res1, bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs, p,
                                         colB, row, b_idx, row_ok, row_valid, st, unit_acc);
-  }
-}
-
-// Tiles whose unit count is odd (192 columns = 3 heads: QKV at batch 1) would leave one group of 4 warps with twice
-// the work of the other; here group g takes the HALF-g chunk (32 columns) of EVERY unit instead — equal work, and each
-// thread needs only its half of the RoPE table (cs[16 g .. 16 g + 16)).  No second output / unit statistics in this
-// mode (bf16 outputs only); staging buffers alternate per unit.
-template <int BN, int ACT, bool OUT_BF16, bool ROPE, int HALF>
-__device__ __forceinline__ void epi_drain_tile_half(uint32_t tmem_acc, const float* bias_s, const float* gate_s,
-                                                    const float* aux_s, const float2 (&cs)[ROPE ? 32 : 1],
-                                                    const GemmParams& p, int n0, int row, int b_idx, bool row_ok,
-                                                    bool row_valid, EpiStage& st) {
-  float4 res[2][8];
-  float2 unit_acc = make_float2(0.f, 0.f);
-  epi_load_resid(p, row, n0 + HALF * 32, row_ok, res[0]);
-#pragma unroll
-  for (int cc = 0; cc < BN / 64; ++cc) {
-    const int col = n0 + cc * 64 + HALF * 32;
-    uint32_t acc[32];
-    if (cc + 1 < BN / 64) epi_load_resid(p, row, col + 64, row_ok, res[(cc + 1) & 1]);
-    tmem_ld32(tmem_acc + cc * 64 + HALF * 32, acc);
-    tmem_wait_ld();
-    st.par_base = (cc & 1) ^ HALF;      // staging buffer cc & 1
-    if (col < p.N)
-      epi_apply<ACT, OUT_BF16, ROPE, HALF>(acc, res[cc & 1], bias_s + cc * 64 + HALF * 32, gate_s + cc * 64 + HALF * 32,
-                                           aux_s + cc * 64 + HALF * 32, cs, p, col, row, b_idx, row_ok, row_valid, st, unit_acc);
-  }
-}
-
-// Variant for grids that fit in one wave (one CTA per SM, registers to spare): the residual of the
-// WHOLE tile is requested before the accumulator is awaited, so no residual latency is exposed in
-// the drain loop (the double-buffered variant above still exposes most of an L2 round trip per
-// chunk: its per-chunk work is much shorter than the latency it tries to cover).
-template <int BN, int ACT, bool OUT_BF16, bool ROPE>
-__device__ __forceinline__ void epi_drain_tile_preloaded(uint32_t tmem_acc, const float* bias_s,
-                                                         const float* gate_s, const float* aux_s,
-                                                         const float2 (&cs)[ROPE ? 32 : 1],
-                                                         float4 (&res)[BN / 32][8], const GemmParams& p,
-                                                         int n0, int row, int b_idx, bool row_ok,
-                                                         bool row_valid, EpiStage& st) {
-  float2 unit_acc = make_float2(0.f, 0.f);
-  st.par_base = 0;
-#pragma unroll
-  for (int cc = 0; cc < BN / 64; ++cc) {
-    const int colA = n0 + cc * 64, colB = colA + 32;
-    uint32_t acc[32];
-    tmem_ld32(tmem_acc + cc * 64, acc);
-    tmem_wait_ld();
-    F5_EPI_MARK(1, cc == 0, 3);    // first TMEM load landed
-    if (colA < p.N)
-      epi_apply<ACT, OUT_BF16, ROPE, 0>(acc, res[2 * cc], bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
-                                        b_idx, row_ok, row_valid, st, unit_acc);
-    F5_EPI_MARK(1, cc == 0, 4);    // chunk 0 complete
-    tmem_ld32(tmem_acc + cc * 64 + 32, acc);
-    tmem_wait_ld();
-    if (colB < p.N)
-      epi_apply<ACT, OUT_BF16, ROPE, 1>(acc, res[2 * cc + 1], bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs,
-                                        p, colB, row, b_idx, row_ok, row_valid, st, unit_acc);
   }
 }
 

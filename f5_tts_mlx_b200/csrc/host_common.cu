@@ -21,9 +21,8 @@ int set_error(int code, const char* fmt, ...) {
 bool pdl_enabled() {
   static int on = -1;
   if (on < 0) {
-    // measured on B200 (bench.py, B=1) with the trigger at kernel START: 97.9 ms/step vs 92.0 without
-    // (the dependent grid became resident too early); the trigger now sits at the start of each
-    // kernel's epilogue: 65.9 vs 67.4 ms/step at B=1, neutral at B=64.  F5_PDL=0 disables.
+    // the trigger sits at the start of each kernel's epilogue (a trigger at kernel start makes the dependent
+    // grid resident too early and takes SMs from the running one).  F5_PDL=0 disables.
     const char* v = getenv("F5_PDL");
     on = (v && v[0] == '0') ? 0 : 1;
   }
@@ -33,10 +32,10 @@ bool pdl_enabled() {
 int sm_count() {
   static int cache[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev >= 0 && dev < 64 && cache[dev] > 0) return cache[dev];
   int sms = 0;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   if (dev >= 0 && dev < 64) cache[dev] = sms;
   return sms;
 }
@@ -52,9 +51,9 @@ int device_check() {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10)
+  if (major != 9)
     return set_error(F5_ERR_NO_DEVICE,
-                     "device %d is sm_%d%d; libf5b200 is built for sm_100a only", dev, major,
+                     "device %d is sm_%d%d; libf5b200 is built for sm_90a only", dev, major,
                      minor);
   return 0;
 }

@@ -26,7 +26,7 @@ int set_error(int code, const char* fmt, ...);
     if (!(cond)) return f5::set_error(F5_ERR_INVALID, __VA_ARGS__);  \
   } while (0)
 
-// 0 if an sm_100 device is current, else F5_ERR_NO_DEVICE (message set)
+// 0 if an sm_90 device is current, else F5_ERR_NO_DEVICE (message set)
 int device_check();
 
 // bf16 tensor map with 128-byte swizzle and zero OOB fill.  dims/strides innermost first;

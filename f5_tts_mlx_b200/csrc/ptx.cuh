@@ -1,10 +1,8 @@
-// Inline-PTX wrappers for the sm_100a features the kernels in this directory use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences) and the
-// UMMA shared-memory + instruction descriptors.  No CUTLASS/CuTe dependency.
+// Inline-PTX wrappers for the sm_90a features the kernels in this directory use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence / mma_async / commit / wait) and the
+// wgmma shared-memory matrix descriptor.  No CUTLASS/CuTe dependency.
 //
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptor" / "instruction
-// descriptor" tables (cross-checked against cute/arch/mma_sm100_desc.hpp, which documents the
-// same fields).
+// Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" table of the wgmma section.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -30,10 +28,9 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// One thread of a CONVERGED warp.  Choosing it with elect.sync instead of `lane == 0` matters for code size in the
-// single-thread TMA / tcgen05 loops: under `lane == 0` the compiler wraps every UTCHMMA / UTMALDG / UTCBAR in an
-// ELECT + R2UR.BROADCAST + BRA.U.ANY serialisation loop (7 instructions per MMA); under elect.sync they issue
-// back to back.  F5_ELECT_MODE=0 restores lane 0 for A/B measurements.
+// One thread of a CONVERGED warp.  Choosing it with elect.sync instead of `lane == 0` keeps the single-thread TMA
+// loops free of the compiler's per-instruction serialisation loop around uniform-datapath operations.
+// F5_ELECT_MODE=0 restores lane 0 for A/B measurements.
 #ifndef F5_ELECT_MODE
 #define F5_ELECT_MODE 1
 #endif
@@ -45,7 +42,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization
-// attribute may START (barrier init, TMEM alloc, descriptor prefetch) while its predecessor in the
+// attribute may START (barrier init, descriptor prefetch) while its predecessor in the
 // stream is still running; pdl_wait() blocks until the predecessor grid has fully completed and its
 // memory is visible.  Every kernel in this library calls pdl_launch_dependents() first thing and
 // pdl_wait() before its first global-memory access; both are no-ops for ordinary launches.
@@ -82,7 +79,7 @@ __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (TMA / tcgen05.mma operand reads)
+  // make generic-proxy smem writes visible to the async proxy (TMA stores / wgmma operand reads)
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -104,48 +101,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must become a trapped launch error, never a hung GPU
-// (a hang costs the whole GPU box).  ~2e9 cycles ≈ 1 s at 1.9 GHz.
+// Bounded wait: a protocol bug must become a trapped launch error, never a hung GPU.  ~4e9 cycles ≈ 2 s at
+// 1.98 GHz.  No function call (printf) on this path: the wgmma consumers wait between MMA issue and MMA wait, and
+// ptxas serialises every wgmma of a kernel whose wgmma pipeline crosses a call.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
-  long long t0 = clock64();
+  const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && (clock64() - t0) > 4000000000LL) {
-      printf("f5: mbarrier wait timeout (block %d,%d thread %d parity %u)\n", blockIdx.x,
-             blockIdx.y, threadIdx.x, parity);
-      __trap();
-    }
-  }
-}
-
-// The same bounded wait for the single-thread issue / producer loops, on a 32-bit shared address: those warps run on
-// a 40-register budget (setmaxnreg) and every spill in them sits between two MMAs, so the time-out keeps a 32-bit
-// clock and reports out of line.
-__device__ __forceinline__ bool mbar_try_wait_u32(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-static __device__ __noinline__ void mbar_timeout_report(uint32_t bar, uint32_t parity) {
-  printf("f5: mbarrier wait timeout (block %d,%d thread %d barrier 0x%x parity %u)\n", blockIdx.x, blockIdx.y,
-         threadIdx.x, bar, parity);
-}
-__device__ __forceinline__ void mbar_wait_u32(uint32_t bar, uint32_t parity) {
-  if (mbar_try_wait_u32(bar, parity)) return;
-  const uint32_t t0 = (uint32_t)clock();
-  uint32_t spins = 0;
-  while (!mbar_try_wait_u32(bar, parity)) {
-    if ((++spins & 0x3ff) == 0 && (uint32_t)((uint32_t)clock() - t0) > 3500000000u) {   // ~1.8 s
-      mbar_timeout_report(bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3ff) == 0 && (clock64() - t0) > 4000000000LL) asm volatile("trap;");
   }
 }
 
@@ -199,161 +163,80 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit
+// wgmma (warpgroup MMA, sm_90a): D (fp32, registers) (+)= A · B, issued by all 128 threads of a warpgroup.
+// Accumulator fragment of m64nN: thread t (warp w = t / 32 of the warpgroup, lane l) holds d[i] at
+//   row 16 w + l / 4 + 8 ((i / 2) % 2),  column 8 (i / 4) + 2 (l % 4) + i % 2.
+// A fragment of the register-A form (m64k16, bf16): a[m] = the bf16 pair of d[8 kk + 2 m], d[8 kk + 2 m + 1] of an
+// m64nN accumulator for k-step kk — which lets a softmax hand its probabilities straight to the next MMA.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+// the accumulator registers must not be touched by the compiler while an MMA that writes them is in flight
+template <int N>
+__device__ __forceinline__ void wgmma_reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols)
-               : "memory");
+
+// Shared-memory matrix descriptor (sm_90), 128-byte swizzle (layout type 1 in bits [62,64)):
+//   bits [0,14)  start address >> 4          bits [16,30) leading-dim byte offset >> 4
+//   bits [32,46) stride-dim byte offset >> 4  bits [49,52) base offset (0: tiles on 1024-byte boundaries)
+// K-major operand, rows of 128 bytes (64 bf16 / 128 e4m3) as TMA writes them with SWIZZLE_128B: consecutive 8-row
+// groups are 1024 B apart (SBO); LBO is unused.  A K-step inside the 128-byte row advances the start address by
+// 32 bytes (16 bf16 / 32 e4m3).
+// MN-major operand (V[key][d] as the B operand with N = d contiguous, 64 elements = one swizzle span): 8 K-rows per
+// 1024-byte atom, SBO = 1024 B between K-groups, LBO = distance between 64-element MN chunks (unused for N = 64).
+__host__ __device__ constexpr uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 62);
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// commit all previously issued tcgen05.mma of this thread; arrives (count 1) on `bar` when done.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
+
+// D (+)= A[smem desc] · B[smem desc], both K-major; scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_bf16_ss_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-          smem_u32(bar))
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void tc_commit_u32(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16/f16 inputs, fp32 accumulate, issued by ONE thread
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_bf16_ss_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-
-// The same for 8-bit float operands (kind::f8f6f4, K = 32 per instruction): the FP8 weight / activation mode of the
-// block GEMMs (DESIGN.md section 8).  Both operands e4m3 (instruction-descriptor formats 0), fp32 accumulate.
-__device__ __forceinline__ void umma_f8_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                           uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_e4m3_ss_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-
-// D[tmem] (+)= A[tmem] * B[smem desc]: A (M x K, K-major) read from tensor memory — row m in lane m, two
-// 16-bit K elements per 32-bit column (K = 16 -> 8 columns at `tmem_a`)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b,
-                                            uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_e4m3_ss_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};\n" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-
-// tcgen05.ld 32 lanes x 32 bit, x16 / x32 columns: thread t of warp w reads TMEM lane
-// 32*(w%4)+t, columns [col, col+n).  taddr = (lane << 16) | col.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
+__device__ __forceinline__ void wgmma_bf16_rs_n64_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                 "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b));
 }
 
-// ---------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type = 2), descriptor version 1.
-//   bits [0,14)  start address >> 4         bits [16,30) leading-dim byte offset >> 4
-//   bits [32,46) stride-dim byte offset >> 4 bits [46,48) version (1 on sm_100)
-//   bits [49,52) base offset                 bits [61,64) layout type
-// K-major operand, rows of 64 bf16 (=128 B) as TMA writes them with SWIZZLE_128B: consecutive
-// 8-row groups are 1024 B apart (SBO); LBO is unused for swizzled K-major layouts.
-// MN-major operand (e.g. V[kv][d] used as B with N=d contiguous, 64 elements = one 128 B
-// swizzle span): 8 k-rows per 1024 B atom; SBO = 1024 B between k-groups; LBO = distance between
-// 64-element MN chunks (unused when the MN extent is 64).
-__host__ __device__ constexpr uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes,
-                                                    uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // version
-  d |= (uint64_t)2 << 61;  // SWIZZLE_128B
-  return d;
-}
-
-// The descriptor as two words: the high one (SBO, version, swizzle mode) is a compile-time constant of the layout, the
-// low one carries the start address (>> 4, 14 bits: adding a byte offset >> 4 never carries out of it).  The
-// single-thread issue loops keep ONE running 32-bit word per operand ring instead of 64-bit descriptors.
-__device__ __forceinline__ uint64_t umma_desc_words(uint32_t lo, uint32_t hi) {
-  return ((uint64_t)hi << 32) | (uint64_t)lo;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D format (1 = f32)  [7,10) A format (1 = bf16)  [10,13) B format (1 = bf16)
-//   [15] A major (0 = K)      [16] B major (0 = K, 1 = MN)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major,
-                                                       int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) |
-         ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// kind::f8f6f4 with e4m3 A/B (format code 0 in [7,10) and [10,13)), fp32 D; K-major operands
-__host__ __device__ constexpr uint32_t umma_idesc_e4m3(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 // ---------------------------------------------------------------------------------------------
 // small math helpers shared by the epilogues
@@ -380,25 +263,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 2^x for a PAIR of inputs on the FMA/ALU pipes only (no MUFU): round-to-nearest split x = n + f,
-// |f| <= 0.5, degree-3 minimax polynomial for 2^f (max rel. error 7.5e-5, far below the bf16
-// rounding of the probabilities it feeds), 2^n applied by adding n to the exponent field.  Used for
-// a fraction of the softmax exponentials so that the MUFU pipe (16 ex2/clk/SM) stops being the
-// bound of the attention kernel.  Inputs must be <= ~0 and are clamped at -126.
-__device__ __forceinline__ float2 ex2_poly2(float2 x) {
-  const float kMagic = 12582912.f;  // 1.5 * 2^23: adding it leaves round(x) in the low mantissa bits
-  x.x = fmaxf(x.x, -126.f);
-  x.y = fmaxf(x.y, -126.f);
-  const float2 r = __fadd2_rn(x, make_float2(kMagic, kMagic));
-  const float2 n = __fadd2_rn(r, make_float2(-kMagic, -kMagic));
-  const float2 f = __fadd2_rn(x, make_float2(-n.x, -n.y));
-  float2 p = __ffma2_rn(make_float2(0.055171646f, 0.055171646f), f, make_float2(0.24261113f, 0.24261113f));
-  p = __ffma2_rn(p, f, make_float2(0.69326097f, 0.69326097f));
-  p = __ffma2_rn(p, f, make_float2(0.99992806f, 0.99992806f));
-  return make_float2(__int_as_float(__float_as_int(p.x) + (__float_as_int(r.x) << 23)),
-                     __int_as_float(__float_as_int(p.y) + (__float_as_int(r.y) << 23)));
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

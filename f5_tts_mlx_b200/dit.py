@@ -1,7 +1,7 @@
 """DiT — host-side mirror of the reference's `f5_tts_mlx.dit.DiT` (dit.py:331-401).
 
 Same constructor arguments and `__call__(x, cond, text, time, drop_audio_cond, drop_text, mask)`
-signature, torch CUDA tensors instead of mx.arrays.  All arithmetic runs in libf5b200 (sm_100a
+signature, torch CUDA tensors instead of mx.arrays.  All arithmetic runs in libf5b200 (sm_90a
 kernels); this module only owns device buffers and fills the C structs.
 """
 from __future__ import annotations
@@ -157,10 +157,10 @@ class DiT:
                                 conv_layers=conv_layers, text_mask_padding=text_mask_padding)
         self.dim, self.depth = dim, depth
         # AdaLN LayerNorm+modulate folded into the neighbouring GEMM epilogues (default); False keeps the separate
-        # f5_ln_modulate launches (the r01 path — kept for A/B measurements and as a cross-check in the tests)
+        # f5_ln_modulate launches (kept for A/B measurements and as a cross-check in the tests)
         self.fused_adaln = bool(fused_adaln)
-        # FP8 mode — the B200 analogue of the reference's quantised `--q` checkpoints (cfm.py:451-452,510-515): the
-        # QKV and FF1 GEMMs (63 % of a block's FLOPs) run on e4m3 operands (kind::f8f6f4 MMAs): weights quantised per
+        # FP8 mode — the H100 analogue of the reference's quantised `--q` checkpoints (cfm.py:451-452,510-515): the
+        # QKV and FF1 GEMMs (63 % of a block's FLOPs) run on e4m3 operands (e4m3 wgmma): weights quantised per
         # tensor at pack time, activations written as e4m3 by the producing GEMM's epilogue.  Lossy like `--q`; gated
         # by the same derived-drift rule against the oracle's e4m3 emulation (tests/test_gpu_parity.py).
         self.fp8 = bool(fp8)

@@ -96,8 +96,8 @@ def generate(
     frame_bucket: int = 128,
 ):
     """generate.py:113-244.  Extensions: `f5tts` reuses a loaded model; `batch_sentences=True` runs all
-    sentences as ONE ragged `sample()` batch instead of the reference's serial loop (SURVEY §8f row 2;
-    numerically it differs from the serial loop only through the reference's own padding caveat — GRN
+    sentences as ONE ragged `sample()` batch instead of the reference's serial loop
+    (numerically it differs from the serial loop only through the reference's own padding caveat — GRN
     statistics and the ODE on padded frames see the batch-maximum length); `frame_bucket` (default 128 frames) lets
     the sentences of the serial loop share one set of buffers and ONE captured CUDA graph per length bucket instead of
     re-capturing for every distinct length (0 = the exact shapes); results are unchanged (F5TTS.sample)."""
@@ -172,7 +172,7 @@ def generate(
 
 
 def main(argv=None) -> None:
-    p = argparse.ArgumentParser(description="Generate speech from text using F5-TTS on B200")
+    p = argparse.ArgumentParser(description="Generate speech from text using F5-TTS on H100")
     p.add_argument("--model", type=str, default="lucasnewman/f5-tts-mlx")
     p.add_argument("--text", type=str, default=None)
     p.add_argument("--duration", type=float, default=None)

@@ -5,7 +5,7 @@ The path has no per-step collective — utterances never interact (cfm.py:340-36
 weight buffer at load (PackedDiT.broadcast).  Outputs are gathered on the host side.
 
 Caveat kept from the reference: a ragged batch is padded to the batch maximum N, which leaks into
-GRN and into the ODE on padded frames (SURVEY §7).  To reproduce an unsharded ragged batch
+GRN and into the ODE on padded frames.  To reproduce an unsharded ragged batch
 bit-for-bit every shard must pad to the GLOBAL N — `global_frames()` computes it with one
 all-reduce(MAX) of an integer; equal-length batches (all BASELINE configs) never need it.
 """

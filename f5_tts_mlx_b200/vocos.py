@@ -1,10 +1,10 @@
 """Vocos vocoder — host-side stand-in for `vocos_mlx.Vocos` as the reference uses it
 (cfm.py:19,446,471: `vocoder=vocos.decode`, called as `vocoder(out)` on a (b, n, 100) mel at
-cfm.py:399-400).  Arithmetic: libf5b200 `f5_vocos_decode` (tcgen05 GEMMs, dwconv+LN kernel,
+cfm.py:399-400).  Arithmetic: libf5b200 `f5_vocos_decode` (wgmma GEMMs, dwconv+LN kernel,
 warp-shuffle inverse FFT + overlap-add).
 
 vocos-mlx is a third-party package that is not vendored in the reference tree; the architecture
-here is the public Vocos "mel-24khz" design restated in SURVEY.md §8c, and the ISTFT
+here is the public Vocos "mel-24khz" design, and the ISTFT
 normalisation/trim convention is an explicit switch (VocosConfig.istft_norm / istft_trim).
 """
 from __future__ import annotations

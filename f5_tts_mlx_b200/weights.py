@@ -1,7 +1,6 @@
 """Model configs, synthetic (seeded) initialisation and weight packing for the CUDA path.
 
-Parameter dictionaries use the reference's MLX parameter-tree names and layouts (SURVEY.md §8a;
-Linear (out, in), Conv1d (out, k, in/groups)), i.e. exactly what `F5TTS.from_pretrained`
+Parameter dictionaries use the reference's MLX parameter-tree names and layouts (Linear (out, in), Conv1d (out, k, in/groups)), i.e. exactly what `F5TTS.from_pretrained`
 (cfm.py:475-517) feeds `load_weights` after its key conversion.  `pack_dit` turns such a dict into
 the packed device layout libf5b200 consumes (include/f5_b200.h: f5_dit_weights), inside ONE
 contiguous device buffer so that the multi-GPU path is a single broadcast of that buffer.
@@ -212,7 +211,7 @@ def convert_upstream_keys(weights: Weights) -> Weights:
 # input dim is a multiple of 64, `weight` (uint32, `32 // bits` codes per word, code j of a word in bits
 # [j*bits, (j+1)*bits)), `scales` and `biases` (one per group of 64 consecutive input channels):
 #     w[o, i] = scales[o, i // 64] * code[o, i] + biases[o, i // 64]        (mx.dequantize)
-# The B200 path computes in bf16 anyway, so such files are dequantised once at load time (pack time).
+# The H100 path computes in bf16 anyway, so such files are dequantised once at load time (pack time).
 # ---------------------------------------------------------------------------------------------
 MLX_GROUP_SIZE = 64
 

@@ -1,5 +1,5 @@
 /*
- * f5_b200.h — C ABI of libf5b200.so, the B200 (sm_100a) implementation of the f5-tts-mlx hot path.
+ * f5_b200.h — C ABI of libf5b200.so, the H100 (sm_90a) implementation of the f5-tts-mlx hot path.
  *
  * The reference (lucasnewman/f5-tts-mlx) has no FFI/plugin boundary: it is pure Python on MLX, and
  * its "operators" are the mlx.nn / mx.fast calls inside f5_tts_mlx/{cfm,dit,convnext_v2,rope,audio}.py.
@@ -16,11 +16,11 @@
  *     cores ("bf16" below = __nv_bfloat16 bits), fp32 for the residual stream, statistics, softmax
  *     and ODE state.  Linear weights are (out_features, in_features) row-major bf16, exactly the
  *     reference's nn.Linear.weight layout.
- *   - there is NO CPU fallback: if no sm_100 device is present every compute entry point fails with
+ *   - there is NO CPU fallback: if no sm_90 device is present every compute entry point fails with
  *     F5_ERR_NO_DEVICE.
  */
-#ifndef F5_B200_H_
-#define F5_B200_H_
+#ifndef F5_H100_H_
+#define F5_H100_H_
 
 #include <stddef.h>
 #include <stdint.h>
@@ -32,7 +32,7 @@ extern "C" {
 #define F5_OK 0
 #define F5_ERR_INVALID (-1)   /* bad argument (shape/alignment/null)            */
 #define F5_ERR_CUDA (-2)      /* a CUDA runtime / driver call failed             */
-#define F5_ERR_NO_DEVICE (-3) /* no sm_100 GPU: this library has no CPU path     */
+#define F5_ERR_NO_DEVICE (-3) /* no sm_90 GPU: this library has no CPU path     */
 
 const char* f5_last_error(void);
 /* library/ABI version (major*1000+minor) and the device check used by every entry point */
@@ -59,7 +59,7 @@ int f5_prof_graph_begin(void* slots, int32_t max_slots);
 int f5_prof_graph_meta(int32_t* kinds, double* flops, double* bytes, int32_t cap);
 
 /* ------------------------------------------------------------------------------------------ *
- * Dense / implicit-conv GEMM on tcgen05 tensor cores:  out = epilogue(A · W^T)
+ * Dense / implicit-conv GEMM on wgmma tensor cores:  out = epilogue(A · W^T)
  * Replaces every nn.Linear / nn.Conv1d on the path (dit.py:33-38,77,94-99,136-143,170,249,267,
  * 286,399; convnext_v2.py:35-44) together with the elementwise ops the reference applies to its
  * result (bias, GELU/Mish, RoPE rope.py:94-107, "* mask" dit.py:172-173, AdaLN gate + residual
@@ -98,10 +98,10 @@ typedef struct f5_gemm_args {
   int32_t rope_cols;      /* columns [0, rope_cols) are rotated in adjacent pairs               */
   float q_scale;          /* columns [0, q_cols) are multiplied by q_scale after the rotation   */
   int32_t q_cols;
-  int32_t tile_n;         /* 0 = auto, else 64 | 128 (single-CTA kernel), 128 | 256 (CTA-pair)   */
+  int32_t tile_n;         /* 0 = auto, else 64 | 128 (192 | 256 are accepted and run as 128)     */
   void* out2_bf16;        /* optional second copy of the result as bf16 [rows, ldo2], or NULL    */
   int64_t ldo2;
-  int32_t variant;        /* 0 auto | 1 single-CTA 128xBN tiles | 2 persistent CTA-pair 256xBN    */
+  int32_t variant;        /* 0 | 1 | 2, kept for ABI compatibility: sm_90 has one 128xBN kernel   */
   int32_t w_static;       /* nonzero: `w` is never written by work that precedes this call on the stream
                              (model weights): the kernel may start fetching it before its programmatic
                              dependency on the preceding kernel has resolved                           */
@@ -123,7 +123,7 @@ typedef struct f5_gemm_args {
   const float* ln_in_stats;
   const float* ln_tab;
   int64_t ln_tab_ld;
-  /* FP8 mode (the B200 analogue of the reference's quantised `--q` checkpoints, cfm.py:451-452,510-515): with ab_fp8
+  /* FP8 mode (the H100 analogue of the reference's quantised `--q` checkpoints, cfm.py:451-452,510-515): with ab_fp8
    * both `a` and `w` hold e4m3 bytes (lda / ldw in elements = bytes, multiples of 16; k a multiple of 128) and the
    * accumulator is multiplied by acc_scale (the weight tensor's quantisation scale, > 0) before bias / LN terms;
    * with out2_fp8 the second output out2_bf16 is written as e4m3 bytes (ldo2 in bytes) — the A operand of the next
@@ -153,8 +153,7 @@ int f5_attention_fwd(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out,
 int f5_attention_fwd_e4m3(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch,
                           int32_t frames, int32_t heads, int32_t head_dim, const int32_t* kv_len,
                           void* stream);
-/* debug aid: while `base` is non-NULL, attention launches write SM-clock stamps of CTA (0,0,0) into it:
-   uint64 [3 roles (softmax group 0, group 1, MMA warp)][64 key tiles][8 slots]; NULL switches it off. */
+/* kept for ABI compatibility: accepts any `base` and returns 0; the attention kernel records no timeline */
 int f5_debug_attention_ts(void* base);
 
 /* ------------------------------------------------------------------------------------------ *
@@ -181,7 +180,7 @@ int f5_grn(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gam
  * DiT (dit.py:331-401) and the ODE loop of F5TTS.sample (cfm.py:340-393).
  *
  * Weight layout ("packed"): what f5_tts_mlx_b200.weights.pack_dit() produces from the MLX
- * parameter tree (SURVEY.md §8a): Linear weights bf16 (out,in); q/k/v fused row-wise into one
+ * parameter tree: Linear weights bf16 (out,in); q/k/v fused row-wise into one
  * [3D, D] matrix; the per-block AdaLN linears (dit.py:263,282) concatenated row-wise into one
  * [depth*6D + 2D, D] matrix so the modulation vectors of ALL ODE time points are one GEMM; the
  * grouped k=31 convs (dit.py:33-38) as [D, 31*64] tap-major block-diagonal-by-64; the input
@@ -403,7 +402,7 @@ int f5_vocos_decode(const f5_vocos_weights* w, const f5_vocos_buffers* b, const 
  *                      then f5_bind_packed_weights on the device copy).
  * f5_bind_workspace  : carves f5_dit_buffers out of one 256-byte-aligned device block of f5_workspace_bytes(), zeroes
  *                      it and uploads the RoPE table; the caller then fills text / text_len / seq_len / cond / tvals.
- * f5_nccl_broadcast_weights : ncclBroadcast of the packed buffer from `root` (SURVEY 8e: "a single NCCL broadcast of
+ * f5_nccl_broadcast_weights : ncclBroadcast of the packed buffer from `root` ("a single NCCL broadcast of
  *                      weights at load, no per-step collective"); `nccl_comm` is an initialised ncclComm_t; the NCCL
  *                      symbol is taken from the library already loaded in the process (or libnccl.so.2).
  * ------------------------------------------------------------------------------------------ */
@@ -430,4 +429,4 @@ int f5_nccl_broadcast_weights(void* device_buf, int64_t bytes, int32_t root, voi
 #ifdef __cplusplus
 }
 #endif
-#endif /* F5_B200_H_ */
+#endif /* F5_H100_H_ */

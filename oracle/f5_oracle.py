@@ -6,7 +6,7 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl
 may import this module.  The product package (f5_tts_mlx_b200) never does.
 
 PARITY UNPINNED: the reference ships no tests, golden vectors or fixtures for this path
-(SURVEY.md §4, §8c) and its runtime (mlx, vocos-mlx) is not installable in this image, so this
+and its runtime (mlx, vocos-mlx) is not installable in this image, so this
 restatement cannot be checked against outputs of the reference itself.  It is pinned instead
 against independent library implementations of the same operators (torchaudio MelSpectrogram,
 torch.nn.functional conv1d / layer_norm / scaled_dot_product_attention / gelu / mish, torch.istft)
@@ -18,7 +18,7 @@ recomputed on every forward, AdaLN linears recomputed per block per forward, ful
 because the same code is the CPU baseline that bench.py times.
 
 Weights are a flat dict name -> torch.Tensor using the MLX parameter-tree names and MLX layouts
-(Linear: (out, in); Conv1d: (out, k, in/groups)), see SURVEY.md §8a.
+(Linear: (out, in); Conv1d: (out, k, in/groups)).
 
 `emulate_bf16=True` rounds every tensor-core operand (GEMM/conv inputs and weights, q/k/v, softmax
 probabilities, attention output) to bf16 while accumulating in fp32 — the precision model of the
@@ -179,7 +179,7 @@ def stft(x: Tensor, window: Tensor, nperseg: int, noverlap: int) -> Tensor:
 
 
 def log_mel_spectrogram(audio: Tensor, sample_rate=24_000, n_mels=100, n_fft=1024, hop_length=256) -> Tensor:
-    """audio.py:162-210 — returns (b, frames, n_mels) (frames-major, see SURVEY §8a13)."""
+    """audio.py:162-210 — returns (b, frames, n_mels) (frames-major)."""
     if audio.ndim == 1:
         audio = audio[None]
     filters = mel_filters(sample_rate, n_fft, n_mels)
@@ -337,7 +337,7 @@ def input_embedding(x: Tensor, cond: Tensor, text_embed: Tensor, drop_audio_cond
 def attention(x: Tensor, mask: Optional[Tensor], rope: Tensor, W: Weights, pfx: str, heads: int,
               prec: Precision = FP32, adaln: Optional[Tuple[Tensor, Tensor]] = None) -> Tensor:
     """dit.py:126-175.  `mask` (b, n) bool = key-padding mask with the INTENDED semantics of
-    dit.py:161-166 (the reference's `.expand` call is not an mx.array method, SURVEY §8c)."""
+    dit.py:161-166 (the reference's `.expand` call is not an mx.array method)."""
     b, n, _ = x.shape
     if adaln is not None:   # x is the un-normalised stream; AdaLayerNormZero (dit.py:270) feeds to_q/k/v (dit.py:313-316)
         s8 = None
@@ -420,7 +420,7 @@ def dit_forward(x: Tensor, cond: Tensor, text: Tensor, time: Tensor, drop_audio_
 
 
 # ---------------------------------------------------------------------------------------------
-# duration.py — DurationPredictor (SURVEY §8f "next" row 1): runs once before the ODE loop when
+# duration.py — DurationPredictor: runs once before the ODE loop when
 # `duration=None` (cfm.py:253-262, 307-308).
 # ---------------------------------------------------------------------------------------------
 @dataclass
@@ -583,7 +583,7 @@ def sample(cond: Tensor, text, duration, W: Weights, cfg: DiTConfig, *, lens: Op
     """cfm.py:264-402.  Returns (out, trajectory) exactly like the reference.
 
     `y0` injects the initial noise (b, N, 100): MLX's threefry stream cannot be reproduced without
-    MLX, so "identical seeds" parity is defined on injected noise (SURVEY §8c).  Without `y0` a
+    MLX, so "identical seeds" parity is defined on injected noise.  Without `y0` a
     torch generator is seeded per element like cfm.py:369-375 (same seed for every element, noise
     drawn as (100, dur) then transposed)."""
     prep = sample_prologue(cond, text, duration, W, lens=lens, vocab_char_map=vocab_char_map,
@@ -621,7 +621,7 @@ def dit_forwards_per_sample(steps: int, method: str, cfg_strength: float) -> int
 
 # ---------------------------------------------------------------------------------------------
 # Vocos (third-party vocos-mlx, NOT in /root/reference; call sites cfm.py:19,399-400,446,471).
-# Restated from the public Vocos "mel-24khz" design (SURVEY §8c): ConvNeXt backbone + ISTFT head.
+# Restated from the public Vocos "mel-24khz" design: ConvNeXt backbone + ISTFT head.
 # Parity of this block is against this oracle only.
 # ---------------------------------------------------------------------------------------------
 @dataclass
@@ -689,7 +689,7 @@ def vocos_decode(mel: Tensor, W: Weights, vc: VocosConfig = VocosConfig(), prec:
 
 
 # ---------------------------------------------------------------------------------------------
-# FLOP accounting (SURVEY §8d) — used by bench.py for the roofline
+# FLOP accounting — used by bench.py for the roofline
 # ---------------------------------------------------------------------------------------------
 def dit_forward_flops(n: int, cfg: DiTConfig) -> float:
     D, L = cfg.dim, cfg.depth

@@ -12,7 +12,7 @@ int main(void) {
   printf("abi=%d structs=%d sizeof(f5_gemm_args)=%d/%d\n", f5_abi_version(), n, (int)sizeof(f5_gemm_args), (int)sizes[0]);
   if (n != 10 || (int)sizeof(f5_gemm_args) != sizes[0]) return 1;   /* the C compiler's layout == the library's */
   int rc = f5_device_check();
-  printf("device_check=%d (%s)\n", rc, rc ? f5_last_error() : "sm_100 device present");
+  printf("device_check=%d (%s)\n", rc, rc ? f5_last_error() : "sm_90 device present");
   f5_gemm_args g;
   memset(&g, 0, sizeof g);
   int rg = f5_gemm_bf16(&g, NULL);      /* no device: F5_ERR_NO_DEVICE; with a device: rejected as invalid (null operands) */

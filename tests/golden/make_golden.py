@@ -76,7 +76,7 @@ np.savez_compressed(os.path.join(HERE, "vocos_small.npz"), mel=mel.numpy(), wave
 for f in sorted(os.listdir(HERE)):
     print(f, os.path.getsize(os.path.join(HERE, f)))
 
-# (f) DurationPredictor (SURVEY §8f row 1)
+# (f) DurationPredictor
 from f5_tts_mlx_b200.weights import random_duration_weights  # noqa: E402
 dW = random_duration_weights(seed=777)
 dWo = {"duration." + k: v for k, v in dW.items()}
@@ -89,7 +89,7 @@ np.savez_compressed(os.path.join(HERE, "duration_small.npz"), mel=mel.numpy(), t
                     seconds=sec.numpy(), weight_seed=777)
 print("duration", sec)
 
-# (g) per-operator input/output pairs (SURVEY §8c item 4) on a small DiT (dim 128, 2 heads, 1 block)
+# (g) per-operator input/output pairs on a small DiT (dim 128, 2 heads, 1 block)
 from f5_tts_mlx_b200.weights import DiTConfig as PkgDiTConfig                     # noqa: E402
 tiny = PkgDiTConfig(dim=128, depth=1, heads=2, ff_mult=2, text_dim=64, conv_layers=1, text_num_embeds=50)
 tcfg = O.DiTConfig(dim=128, depth=1, heads=2, ff_mult=2, text_num_embeds=50, text_dim=64, conv_layers=1)

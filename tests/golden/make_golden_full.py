@@ -24,7 +24,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-N10S, NREF10S, NTEXT = 937, 328, 152          # SURVEY §8d synthetic 10 s utterance
+N10S, NREF10S, NTEXT = 937, 328, 152          # synthetic 10 s utterance
 CFG3_BATCH, CFG3_CHECKED = 64, (0, 37)        # config 3: 64 equal-length utterances; oracle on two of them
 N60S, NREF60S, NTEXT60S = 5625, 499, 900      # config 5: 60 s, text longer than... positions clamp at 4095 is exercised by N > 4096
 
@@ -126,8 +126,10 @@ def main():
             fwd16 = O.dit_forward(y0, prep.step_cond, prep.text, tt, False, False, None, W, ocfg, emu)
         drift = _rel(out16[:, NREF60S:], out[:, NREF60S:])
         # every 3rd frame of the sample keeps the file small (the forward is stored in full as fp16-safe fp32)
-        np.savez_compressed(os.path.join(HERE, "full_cfg5_long.npz"), out_sub3=out[0, ::3].numpy(), drift=np.float64(drift),
-                            fwd_sub3=fwd[0, ::3].numpy(), fwd_drift=np.float64(_rel(fwd16, fwd)), weight_seed=1234,
+        # float16 storage keeps the file under 1 MB; its rounding (2e-4 relative) is far below the test's tolerance
+        np.savez_compressed(os.path.join(HERE, "full_cfg5_long.npz"), out_sub3=out[0, ::3].numpy().astype(np.float16),
+                            drift=np.float64(drift), fwd_sub3=fwd[0, ::3].numpy().astype(np.float16),
+                            fwd_drift=np.float64(_rel(fwd16, fwd)), weight_seed=1234,
                             input_seed=50505, input_checksum=input_checksum(cond, text, y0))
         print(f"cfg5: {time.time() - t0:.0f}s drift={drift:.3e} fwd drift={_rel(fwd16, fwd):.3e}", flush=True)
     for f in sorted(os.listdir(HERE)):

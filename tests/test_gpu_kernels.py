@@ -226,7 +226,7 @@ def test_gemm_fused_ln_consumer(M, D, N, act, rope):
     assert rel(out, ref) < 6e-3
 
 
-# ---------------- FP8 mode (e4m3 operands, kind::f8f6f4) ----------------
+# ---------------- FP8 mode (e4m3 operands, e4m3 wgmma) ----------------
 def _e4m3(x):
     return x.clamp(-448, 448).to(torch.float8_e4m3fn)
 

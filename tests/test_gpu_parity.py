@@ -259,7 +259,7 @@ def test_end_to_end_raw_wave_to_waveform(gate):
     assert rel(wave.cpu(), ref) < 3e-2
 
 
-# ---------------- DurationPredictor (SURVEY §8f row 1) ----------------
+# ---------------- DurationPredictor ----------------
 def test_duration_predictor_vs_oracle_and_golden(golden_dir):
     from f5_tts_mlx_b200.duration import DurationPredictor, DurationTransformer
     from f5_tts_mlx_b200.weights import random_duration_weights
@@ -349,11 +349,11 @@ def test_generate_end_to_end_serial_and_batched_sentences(tmp_path):
 
 # ---------------- multi-GPU: sharded == unsharded (needs 2 GPUs; skipped on a 1-GPU box) ----------------
 def test_nccl_sharded_ragged_batch_equals_unsharded():
-    """SURVEY §8e: utterances shard across ranks with ONE NCCL weight broadcast and no per-step collective; a ragged
+    """Utterances shard across ranks with ONE NCCL weight broadcast and no per-step collective; a ragged
     batch sharded over 2 GPUs (each shard padded to the global frame count) reproduces the unsharded batch."""
     import json, subprocess, sys
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
                         "--master-addr", "127.0.0.1", "--master-port", "29731",
@@ -492,7 +492,7 @@ def test_frame_bucketing_one_plan_for_many_lengths_same_results(gate):
 
 def test_fp8_mode_forward_within_derived_drift(base):
     """DiT(fp8=True): the four GEMMs of every block on e4m3 operands (weights quantised per tensor at pack time,
-    activations written as e4m3 by the producing kernels) — the B200 analogue of the reference's lossy `--q`
+    activations written as e4m3 by the producing kernels) — the H100 analogue of the reference's lossy `--q`
     checkpoints.  Same rule as everywhere: within 3x the drift of the oracle's emulation of exactly these rounding
     points (Precision(fp8=True)), which is ~7x the bf16 drift."""
     cfg, W, model = base

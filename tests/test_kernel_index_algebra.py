@@ -35,30 +35,32 @@ def test_epilogue_staging_swizzle_is_a_bijection_and_stores_are_coalesced(out_bf
         assert len(rows) == 1
 
 
-# ---- gemm2_sm100.cuh / gemm_epilogue.cuh: two epilogue groups interleave 64-column units ------------------------
-@pytest.mark.parametrize("bn", [128, 192, 256])
-def test_pair_kernel_epilogue_groups_cover_every_column_once(bn):
-    cover = np.zeros(bn, dtype=int)
-    per_group = []
-    for grp in range(2):
-        units = list(range(grp, bn // 64, 2))               # epi_drain_tile(cc0 = grp, cc_step = 2)
-        per_group.append(len(units))
-        for cc in units:
-            cover[cc * 64:(cc + 1) * 64] += 1
-    assert (cover == 1).all()
-    assert max(per_group) - min(per_group) <= 1             # 2+1 units at BN=192, even otherwise
-
-
 def test_single_cta_epilogue_groups_split_the_tile_in_halves():
-    bn, groups = 128, 2                                     # GemmEpi<128, 6>
+    bn, groups = 128, 2                                     # GemmEpi<128>
     cols = [list(range(g * (bn // groups), (g + 1) * (bn // groups))) for g in range(groups)]
     assert sorted(sum(cols, [])) == list(range(bn))
-    # warps 2-5 and 6-9 both cover the four TMEM lane quarters (warp % 4)
-    for first in (2, 6):
-        assert sorted(w % 4 for w in range(first, first + 4)) == [0, 1, 2, 3]
+    # consumer warpgroups 1-2 (threads 128..383) are the two groups; thread & 127 is the tile row in both
+    for g in range(groups):
+        threads = range(128 * (g + 1), 128 * (g + 2))
+        assert {(t >> 7) - 1 for t in threads} == {g}
+        assert sorted(t & 127 for t in threads) == list(range(128))
 
 
-# ---- gemm_sm100.cuh: weight tiles requested before the PDL wait --------------------------------------------------
+# ---- gemm_sm90.cuh: wgmma accumulator fragments -> the shared-memory accumulator tile ------------------------------
+@pytest.mark.parametrize("bn", [64, 128])
+def test_accumulator_fragments_fill_the_shared_tile_exactly_once(bn):
+    cover = np.zeros((128, bn), dtype=int)
+    for t in range(128, 384):                               # consumer threads
+        wg, warp, lane = (t >> 7) - 1, (t >> 5) & 3, t & 31
+        r = wg * 64 + warp * 16 + (lane >> 2)
+        c = 2 * (lane & 3)
+        for j in range(bn // 8):                            # acc[4j], acc[4j+1] -> row r; acc[4j+2], acc[4j+3] -> row r+8
+            for rr in (r, r + 8):
+                cover[rr, 8 * j + c:8 * j + c + 2] += 1
+    assert (cover == 1).all()
+
+
+# ---- gemm_sm90.cuh: weight tiles requested before the PDL wait --------------------------------------------------
 @pytest.mark.parametrize("num_kb,stages", [(16, 6), (32, 6), (2, 6), (16, 3), (1, 4)])
 def test_early_weight_tiles_plus_main_loop_issue_every_k_block_once(num_kb, stages):
     early_b = min(stages, num_kb)
@@ -72,97 +74,3 @@ def test_early_weight_tiles_plus_main_loop_issue_every_k_block_once(num_kb, stag
         a_loads.append(kb)
     assert b_loads == list(range(num_kb)) and a_loads == list(range(num_kb)) and expect == list(range(num_kb))
     assert all(kb % stages == kb for kb in range(early_b))  # early tiles land in the stage the loop will use
-
-
-# ---- attention2_sm100.cuh: P written to TMEM as the A operand of the TS-form MMA ---------------------------------
-def test_attention_p_tiles_fill_the_tmem_columns_the_mma_reads():
-    # softmax thread: chunk c (8 probabilities) -> 4 packed bf16x2 words; chunks (2q, 2q+1) stored by one
-    # tcgen05.st.x8 at column offset q*8.  MMA k-step k (16 keys) reads columns [k*8, k*8+8).
-    col_of_key = {}
-    for c in range(16):
-        for w in range(4):
-            col = (c >> 1) * 8 + (c & 1) * 4 + w
-            for half in range(2):
-                key = c * 8 + 2 * w + half
-                assert key not in col_of_key
-                col_of_key[key] = (col, half)                # low half = even key (pack_bf16x2(lo, hi))
-    assert sorted(col_of_key) == list(range(128))
-    for k in range(8):
-        keys = [key for key, (col, _) in col_of_key.items() if k * 8 <= col < k * 8 + 8]
-        assert sorted(keys) == list(range(16 * k, 16 * k + 16))
-    for key, (col, half) in col_of_key.items():
-        assert col == key // 2 and half == key % 2           # K-major: two consecutive keys per 32-bit column
-    # TMEM map: S0 S1 O0 O1 P0 P1 = exactly the 512 columns of an SM
-    regions = [(0, 128), (128, 128), (256, 64), (320, 64), (384, 64), (448, 64)]
-    assert sum(n for _, n in regions) == 512
-    assert all(regions[i][0] + regions[i][1] == regions[i + 1][0] for i in range(5))
-
-
-# ---- attention2_sm100.cuh: hand-off barriers between the two softmax groups --------------------------------------
-@pytest.mark.parametrize("num_kv", [1, 2, 3, 8, 9])
-@pytest.mark.parametrize("mode", [1, 2])
-def test_attention_handoff_barriers_are_balanced_and_order_the_groups(num_kv, mode):
-    """bar 2: group 0 syncs, group 1 arrives; bar 3: group 1 syncs, group 0 arrives.  A sync may only complete when
-    a matching arrive has been posted; no arrive may be left unconsumed at exit."""
-    pending = {2: 0, 3: 0}
-    pending[2] += 1                                          # group 1's initial arrive: group 0 goes first
-    pc = {0: 0, 1: 0}                                        # next tile of each group
-    waiting = {0: True, 1: True}                             # at the sync in front of the exponential loop
-    order = []
-    for _ in range(4 * num_kv + 4):
-        progressed = False
-        for g, bar, other_bar in ((0, 2, 3), (1, 3, 2)):
-            if pc[g] < num_kv and waiting[g] and pending[bar] > 0:
-                pending[bar] -= 1
-                order.append((g, pc[g]))
-                # exponential loop; the release is at half time (mode 2) or at the end (mode 1) — same counts
-                if g == 0 or pc[g] + 1 < num_kv:
-                    pending[other_bar] += 1
-                pc[g] += 1
-                progressed = True
-        if not progressed:
-            break
-    assert pc == {0: num_kv, 1: num_kv}, "a group starved (deadlock)"
-    assert pending == {2: 0, 3: 0}, "an arrive was left unconsumed at exit"
-    assert order == [(g, j) for j in range(num_kv) for g in (0, 1)]   # strict alternation 0,1,0,1,...
-
-
-def _tile_walk(cluster_id, num_clusters, n_tiles, total_tiles):
-    """Python restatement of gemm2_sm100.cuh tile_walk()."""
-    m_tiles = total_tiles // n_tiles
-    G = num_clusters // m_tiles if m_tiles > 0 else 0
-    sticky = total_tiles > num_clusters and G >= 1 and -(-n_tiles // G) <= -(-total_tiles // num_clusters)
-    if sticky:
-        m, j = divmod(cluster_id, G)
-        first, stride = m * n_tiles + j, G
-        count = -(-(n_tiles - j) // G) if (m < m_tiles and j < n_tiles) else 0
-    else:
-        first, stride = cluster_id, num_clusters
-        count = -(-(total_tiles - cluster_id) // num_clusters) if cluster_id < total_tiles else 0
-    return first, stride, count, sticky
-
-
-def test_pair_gemm_tile_walk_covers_every_tile_once_and_row_sticky_keeps_rows():
-    """The persistent CTA-pair GEMM's tile walk: every tile exactly once for any (clusters, n_tiles, m_tiles); in the
-    row-sticky mode (QKV at batch 1: 8 x 16 tiles on 74 clusters) all tiles of a cluster share the row block and
-    no cluster gets more tiles than with the round-robin walk."""
-    seen_sticky = False
-    for clusters in (1, 2, 7, 64, 74):
-        for n_tiles in (1, 2, 4, 12, 16, 24):
-            for m_tiles in (1, 2, 8, 9, 75, 469):
-                total = n_tiles * m_tiles
-                launched = min(clusters, total)
-                tiles, per = [], []
-                for c in range(launched):
-                    first, stride, count, sticky = _tile_walk(c, launched, n_tiles, total)
-                    mine = [first + i * stride for i in range(count)]
-                    tiles += mine
-                    per.append(len(mine))
-                    if sticky:
-                        seen_sticky = True
-                        assert len({t // n_tiles for t in mine}) <= 1
-                assert sorted(tiles) == list(range(total)), (clusters, n_tiles, m_tiles)
-                assert max(per) <= -(-total // launched)
-    assert seen_sticky
-    first, stride, count, sticky = _tile_walk(10, 74, 16, 128)
-    assert sticky and (first, stride, count) == (1 * 16 + 1, 9, 2)

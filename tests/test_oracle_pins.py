@@ -45,7 +45,7 @@ def test_mel_golden_fixture(golden_dir):
     got = O.log_mel_spectrogram(x)[0].numpy()
     assert got.shape == z["mel"].shape == (93, 100)
     np.testing.assert_allclose(got, z["mel"], atol=2e-5)
-    # the whole reference clip (wave module: 127985 samples) -> 499 frames (SURVEY §2 #16)
+    # the whole reference clip (wave module: 127985 samples) -> 499 frames
     assert int(z["full_clip_samples"]) == 127985 and int(z["full_clip_frames"]) == 499
 
 
@@ -217,7 +217,7 @@ def test_vocos_golden(golden_dir):
     assert w2.shape == (11 * 256,) and rel(w2, torch.from_numpy(z["wave_window_sq_trim"])) < 5e-5
 
 
-# ---------------- DurationPredictor restatement (SURVEY §8f row 1) ----------------
+# ---------------- DurationPredictor restatement ----------------
 def test_duration_predictor_golden_and_structure(golden_dir):
     from f5_tts_mlx_b200.weights import random_duration_weights
     z = np.load(os.path.join(golden_dir, "duration_small.npz"))
@@ -237,7 +237,7 @@ def test_duration_predictor_golden_and_structure(golden_dir):
 
 
 def test_per_operator_known_answers(golden_dir):
-    """SURVEY §8c item 4: per-operator input/output pairs (tiny DiT: dim 128, 2 heads, 1 block), generated by
+    """per-operator input/output pairs (tiny DiT: dim 128, 2 heads, 1 block), generated by
     tests/golden/make_golden.py section (g).  Pins every building block of the oracle separately, so a regression is
     localised to the operator, not just visible in the end-to-end fixtures."""
     from f5_tts_mlx_b200.weights import DiTConfig as PkgDiTConfig
