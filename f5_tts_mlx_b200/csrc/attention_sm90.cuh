@@ -50,9 +50,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p)
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int HD = p.H * 64;
-  int kv_len = p.kv_len ? p.kv_len[b] : p.N;
-  kv_len = min(max(kv_len, 1), p.N);
-  const int num_kv = (kv_len + 127) >> 7;
 
   if (warp == 0 && F5_ELECT_LANE()) {
     tma_prefetch_desc(&tma_qkv);
@@ -68,6 +65,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p)
   __syncthreads();
   pdl_wait();
   if (threadIdx.x == 128) prof_stamp_begin(p.prof);   // a consumer thread, not the producer
+  // kv_len is global memory a predecessor may write: read only after the wait
+  int kv_len = p.kv_len ? p.kv_len[b] : p.N;
+  kv_len = min(max(kv_len, 1), p.N);
+  const int num_kv = (kv_len + 127) >> 7;
 
   if (warp < 4) {
     // ===================== TMA producer =====================

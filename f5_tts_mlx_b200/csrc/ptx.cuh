@@ -44,8 +44,10 @@ __device__ __forceinline__ bool elect_one() {
 // programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization
 // attribute may START (barrier init, descriptor prefetch) while its predecessor in the
 // stream is still running; pdl_wait() blocks until the predecessor grid has fully completed and its
-// memory is visible.  Every kernel in this library calls pdl_launch_dependents() first thing and
-// pdl_wait() before its first global-memory access; both are no-ops for ordinary launches.
+// memory is visible.  Every kernel in this library calls pdl_wait() before its first global-memory access
+// (prefetches, and the first weight tiles of a GEMM whose W is static, excepted).  The elementwise and audio kernels
+// call pdl_launch_dependents() first thing, the GEMM and the attention after their main loop.  Both are no-ops for
+// ordinary launches.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() {

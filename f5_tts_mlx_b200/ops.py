@@ -64,8 +64,11 @@ def gemm(
     acc_scale: float = 1.0,                    # multiplies the accumulator in FP8 mode (weight tensor scale)
     out2_fp8: bool = False,                    # out2 is written as e4m3 bytes (uint8 tensor)
     out_fp8: bool = False,                     # out (a uint8 tensor) is written as e4m3 bytes
+    w_static: bool = False,                    # w is not written by the preceding kernel: its first tiles load before the PDL wait
+    prefetch: torch.Tensor | None = None,      # weights of a later GEMM to pull into L2 while this one runs
+    prefetch_bytes: int = 0,
 ) -> torch.Tensor:
-    _need_cuda(a, w, out, bias, resid, gate, row_len, rope, out2, ln_scale, ln_stats, ln_in_stats, ln_tab)
+    _need_cuda(a, w, out, bias, resid, gate, row_len, rope, out2, ln_scale, ln_stats, ln_in_stats, ln_tab, prefetch)
     if ab_fp8:
         a = a.view(torch.uint8) if a.dtype != torch.uint8 else a
         w = w.view(torch.uint8) if w.dtype != torch.uint8 else w
@@ -107,6 +110,10 @@ def gemm(
     if debug_ts is not None:
         g.debug_ts = debug_ts.data_ptr()
     g.ab_fp8, g.acc_scale, g.out2_fp8 = int(ab_fp8), float(acc_scale), int(out2_fp8)
+    g.w_static = int(w_static)
+    if prefetch is not None:
+        assert prefetch_bytes <= prefetch.numel() * prefetch.element_size()
+        g.prefetch, g.prefetch_bytes = prefetch.data_ptr(), prefetch_bytes
     if out2 is not None:
         assert out2.dtype == (torch.uint8 if out2_fp8 else torch.bfloat16) and out2.stride(-1) == 1
         g.out2_bf16, g.ldo2 = out2.data_ptr(), out2.stride(0)

@@ -1,0 +1,288 @@
+"""Element-wise checkers for the GEMM and attention kernels (pure torch, CPU or GPU).
+
+* `assert_exact`: bitwise comparison; a mismatch names the first bad (tile, row, column).
+* `assert_within`: |got - ref| <= bound for every element; returns the worst err/bound ratio and names the tile where
+  it occurs.  The bound helpers below derive per-element bounds from the operation (see their docstrings).
+* `Guarded`: an output view inside a larger buffer pre-filled with a NaN pattern (rows above and below, columns left and
+  right, so ld > n); `check()` asserts that every element of the view was written and every guard element is unchanged.
+
+Tiles are named by a `locate(row, col)` function: `gemm_tiles` for the GEMM's 128 x BN output tiles (flat or batched
+rows), `attn_tiles` for the attention's (batch, head, 128-query tile).
+"""
+from __future__ import annotations
+
+import math
+
+import torch
+
+U32 = 2.0 ** -24          # unit roundoff of fp32 (round to nearest)
+U_BF16 = 2.0 ** -8        # unit roundoff of bf16 (8 significant bits)
+U_E4M3 = 2.0 ** -4        # unit roundoff of e4m3 (4 significant bits)
+E4M3_SUB = 2.0 ** -10     # half the e4m3 subnormal spacing (2^-9): absolute rounding error below 2^-6
+# documented maximum errors of the approximate instructions the epilogues use (PTX ISA / CUDA C Programming Guide)
+EPS_TANH = 2.0 ** -10.987  # tanh.approx.f32: maximum relative error
+EPS_EX2 = 2.0 ** -22       # ex2.approx.ftz.f32: maximum relative error (2 ulp)
+
+_INT = {4: torch.int32, 2: torch.int16, 1: torch.uint8}
+PATTERN = {4: 0x7FA5A5A5, 2: 0x7FA5, 1: 0x7F}   # NaN in fp32 / bf16 / e4m3 (e4m3 0x7F is its only positive NaN)
+
+
+def bits(t: torch.Tensor) -> torch.Tensor:
+    return t.view(_INT[t.element_size()])
+
+
+def e4m3(x: torch.Tensor) -> torch.Tensor:
+    """Round to nearest even e4m3, saturating at +-448: the kernels' cvt.rn.satfinite."""
+    return x.float().clamp(-448, 448).to(torch.float8_e4m3fn)
+
+
+def round_to(ref: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """Round-to-nearest of an fp32-exact float64 reference into the output type."""
+    r32 = ref.float()
+    assert torch.equal(r32.double(), ref.double()), "reference is not exact in fp32"
+    if dtype == torch.float32:
+        return r32
+    if dtype in (torch.uint8, torch.float8_e4m3fn):
+        return e4m3(r32).view(dtype)
+    return r32.to(dtype)
+
+
+def instantiation(*, act: int = 0, out_dtype=torch.bfloat16, rope: bool = False, fp8: bool = False,
+                  resid: bool = False, tile: int, conv_grouped: bool = False) -> tuple:
+    """(ACT, OUT_BF16, ROPE, FP8, RESID, BN) of the gemm_bf16_tn_kernel a launch selects (dispatch_epi in gemm.cu):
+    FP8 when any operand or output is e4m3, RESID = false only for the residual-free GELU-tanh bf16 epilogue, and
+    the grouped convolution always runs 64-column tiles."""
+    out_bf16 = out_dtype != torch.float32
+    no_resid = not resid and act == 1 and out_bf16 and not rope
+    return (act, out_bf16, rope, fp8, not no_resid, 64 if conv_grouped else tile)
+
+
+# ---------------------------------------------------------------- tile naming
+def gemm_tiles(bn: int, rows_per_batch: int = 0, batched: bool = False):
+    """(row, col) -> tile name.  Batched mode: tiles never straddle utterances (tile = (utterance, tile in utterance))."""
+    def locate(row: int, col: int) -> str:
+        if batched:
+            b, r = divmod(row, rows_per_batch)
+            return f"tile (utt {b}, m {r // 128}, n {col // bn}) row {row} col {col}"
+        return f"tile (m {row // 128}, n {col // bn}) row {row} col {col}"
+    return locate
+
+
+def attn_tiles(frames: int, head_dim: int = 64):
+    def locate(row: int, col: int) -> str:
+        b, n = divmod(row, frames)
+        return f"(batch {b}, head {col // head_dim}, q-tile {n // 128}) row {row} col {col}"
+    return locate
+
+
+def _first(mask: torch.Tensor):
+    idx = mask.nonzero()[0].tolist()
+    return idx[0], (idx[1] if len(idx) > 1 else 0)
+
+
+def assert_exact(got: torch.Tensor, want: torch.Tensor, locate, what: str = "") -> None:
+    """Bitwise equality.  `want` has got's dtype (use round_to).  +0 and -0 compare equal: the sign of an exact zero
+    depends on whether the compiler contracts a c - b s into an fma, which is no error."""
+    assert got.shape == want.shape and got.dtype == want.dtype, (got.shape, want.shape, got.dtype, want.dtype)
+    g2, w2 = got.reshape(got.shape[0], -1), want.reshape(want.shape[0], -1)
+    sign = {4: -(2 ** 31), 2: -(2 ** 15), 1: 0x80}[got.element_size()]
+    gb, wb = bits(g2), bits(w2)
+    zero = lambda b: (b | sign) == sign
+    bad = (gb != wb) & ~(zero(gb) & zero(wb))
+    if bad.any():
+        r, c = _first(bad)
+        gv = g2[r, c].float().item() if g2.dtype != torch.uint8 else g2[r, c].view(torch.float8_e4m3fn).float().item()
+        wv = w2[r, c].float().item() if w2.dtype != torch.uint8 else w2[r, c].view(torch.float8_e4m3fn).float().item()
+        raise AssertionError(f"{what}: {int(bad.sum())} elements differ; first at {locate(r, c)}: got {gv!r} want {wv!r}")
+
+
+def assert_within(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor, locate, what: str = "") -> float:
+    """|got - ref| <= bound element-wise (non-finite got fails).  Returns the worst err/bound ratio."""
+    g = got.view(torch.float8_e4m3fn) if got.dtype == torch.uint8 else got
+    g = g.double().reshape(got.shape[0], -1)
+    ref, bound = ref.double().reshape(g.shape), bound.double().reshape(g.shape)
+    assert (bound > 0).all(), f"{what}: bound must be positive"
+    ratio = (g - ref).abs() / bound
+    ratio = torch.where(torch.isfinite(g), ratio, torch.full_like(ratio, math.inf))
+    worst = ratio.max().item()
+    r, c = divmod(int(ratio.argmax()), g.shape[1])
+    msg = (f"{what}: worst err/bound {worst:.3g} at {locate(r, c)}: got {g[r, c].item()!r} ref {ref[r, c].item()!r} "
+           f"bound {bound[r, c].item():.3g}")
+    if not worst <= 1.0:
+        raise AssertionError(msg)
+    print(msg)
+    return worst
+
+
+# ---------------------------------------------------------------- guard regions
+class Guarded:
+    """`view` = rows x cols of `dtype` inside a buffer with `pad_rows` extra rows above and below and at least 16 bytes
+    of extra columns on each side (ld > cols, every row start 16-byte aligned as the TMA stores need).  `lr=False` puts
+    no columns beside the view (contiguous rows, as ln_stats must be)."""
+
+    def __init__(self, rows: int, cols: int, dtype: torch.dtype, device, pad_rows: int = 3, lr: bool = True,
+                 pad_cols: int = 0):
+        esz = torch.empty((), dtype=dtype).element_size()
+        vec = 16 // esz
+        pad = max(vec, (pad_cols + vec - 1) // vec * vec) if lr else 0
+        self.pl = pad
+        ld = self.pl + cols + pad
+        ld = (ld + vec - 1) // vec * vec if lr else ld
+        self.pr, self.rows, self.cols = pad_rows, rows, cols
+        self.buf = torch.empty(rows + 2 * pad_rows, ld, dtype=dtype, device=device)
+        self.pat = PATTERN[esz]
+        bits(self.buf).fill_(self.pat)
+        self.view = self.buf[pad_rows:pad_rows + rows, self.pl:self.pl + cols]
+
+    def check(self, what: str = "") -> None:
+        b = bits(self.buf).long() & ((1 << (8 * self.buf.element_size())) - 1)
+        inside = torch.zeros_like(b, dtype=torch.bool)
+        inside[self.pr:self.pr + self.rows, self.pl:self.pl + self.cols] = True
+        untouched = b == self.pat
+        if (~untouched & ~inside).any():
+            r, c = _first(~untouched & ~inside)
+            raise AssertionError(f"{what}: guard element overwritten at buffer row {r - self.pr} col {c - self.pl} "
+                                 f"(view is rows [0, {self.rows}) cols [0, {self.cols}))")
+        if (untouched & inside).any():
+            r, c = _first(untouched & inside)
+            raise AssertionError(f"{what}: {int((untouched & inside).sum())} elements never written; first at row "
+                                 f"{r - self.pr} col {c - self.pl}")
+
+
+# ---------------------------------------------------------------- references and bounds
+def gemm_acc_bound(a: torch.Tensor, w: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
+    """Bound on the fp32 accumulation error of acc = A W^T (float64 [M, N]).
+
+    Every product of two bf16 (or e4m3) values is exact in fp32.  However the tensor core orders and rounds the K - 1
+    additions, each one adds at most one ulp (truncation instead of round-to-nearest: 2u, u = 2^-24) of a partial sum
+    bounded by sum_k |a_k||w_k|.  So |acc - A W^T| <= 2u (K - 1) / (1 - 2u (K - 1)) (|A||W|^T) < 2u (K + 1) (|A||W|^T)
+    for K < 2^20; the epilogue's fma with bias and acc_scale adds u |v|, charged by the callers."""
+    k = a.shape[-1]
+    return 2 * U32 * (k + 1) * (a.float().double().abs() @ w.float().double().abs().T) * abs(scale)
+
+
+def gemm_acc_bound_fp8(a: torch.Tensor, w: torch.Tensor, scale: float = 1.0) -> torch.Tensor:
+    """The FP8 mode adds each 128-product k-block's e4m3 wgmma partial to the fp32 accumulator on the CUDA cores.  The
+    partial's accumulator is shorter than fp32 and its width is not documented; public measurements of Hopper give
+    about 14 retained bits.  With 13 bits (ulp 2^-12 relative) and one truncating add per 32-product k-step, a block's
+    partial is off by at most 4 * 2^-12 = 2^-10 of the block's sum |products|.  The fp32 promotion of the blocks adds
+    2u per block as in gemm_acc_bound."""
+    kb = a.shape[-1] // 128
+    aa, ww = a.float().double().abs(), w.float().double().abs()
+    full = aa @ ww.T
+    return (2.0 ** -10 + 2 * U32 * (kb + 1)) * full * abs(scale)
+
+
+def rope_ref(x: torch.Tensor, tab: torch.Tensor, pos: torch.Tensor, rope_cols: int) -> torch.Tensor:
+    """Rotate adjacent column pairs (2j, 2j+1) of the first rope_cols columns by the table entry (cos, sin) of the
+    row's position and pair j % 32 of the 64-column head.  x float64 [rows, n]; tab [P, 32, 2]; pos [rows]."""
+    y = x.clone()
+    if rope_cols == 0:
+        return y
+    r = x[:, :rope_cols].reshape(x.shape[0], rope_cols // 64, 32, 2)
+    cs = tab.double()[pos.long()]                      # rows, 32, 2
+    c, s = cs[:, None, :, 0], cs[:, None, :, 1]
+    rot = torch.stack([r[..., 0] * c - r[..., 1] * s, r[..., 1] * c + r[..., 0] * s], -1)
+    y[:, :rope_cols] = rot.reshape(x.shape[0], rope_cols)
+    return y
+
+
+def rope_bound(x: torch.Tensor, bx: torch.Tensor, tab: torch.Tensor, pos: torch.Tensor, rope_cols: int) -> torch.Tensor:
+    """Bound after the rotation of rope_ref, given a bound bx on x: a c - b s moves by |c| bx_a + |s| bx_b, and its fp32
+    evaluation (two products, one subtraction) adds at most 2u (|a c| + |b s|) + u |a c - b s|."""
+    y = bx.clone()
+    if rope_cols == 0:
+        return y
+    n = x.shape[0]
+    xa = x[:, :rope_cols].reshape(n, rope_cols // 64, 32, 2).abs()
+    ba = bx[:, :rope_cols].reshape(n, rope_cols // 64, 32, 2)
+    cs = tab.double()[pos.long()].abs()
+    c, s = cs[:, None, :, 0], cs[:, None, :, 1]
+    e0 = c * ba[..., 0] + s * ba[..., 1] + 3 * U32 * (xa[..., 0] * c + xa[..., 1] * s)
+    e1 = c * ba[..., 1] + s * ba[..., 0] + 3 * U32 * (xa[..., 1] * c + xa[..., 0] * s)
+    y[:, :rope_cols] = torch.stack([e0, e1], -1).reshape(n, rope_cols)
+    return y
+
+
+def _gelu_tanh(v):
+    return 0.5 * v * (1 + torch.tanh(math.sqrt(2 / math.pi) * (v + 0.044715 * v ** 3)))
+
+
+def act_ref(v: torch.Tensor, act: int) -> torch.Tensor:
+    """float64 activations: 0 none, 1 GELU-tanh, 2 GELU-erf, 3 Mish."""
+    v = v.double()
+    if act == 1:
+        return _gelu_tanh(v)
+    if act == 2:
+        return 0.5 * v * (1 + torch.erf(v / math.sqrt(2)))
+    if act == 3:
+        return v * torch.tanh(torch.nn.functional.softplus(v))
+    return v
+
+
+def act_bound(v: torch.Tensor, bv: torch.Tensor, act: int) -> torch.Tensor:
+    """Bound on act(v~) - act(v) for a kernel input v~ with |v~ - v| <= bv, evaluated as the epilogue does.
+
+    Input propagation: |act'| <= 1.13 for GELU (both forms) and <= 1.1 for Mish, everywhere.
+    GELU-tanh = 0.5 x (1 + tanh.approx(u)): tanh.approx's relative error EPS_TANH moves the result by at most
+    0.5 |x| EPS_TANH; the five fp32 operations that form u and the result add at most 6u |x| (|u| <= 0.8 |x| (1 + |x|^2 / 20),
+    whose rounding passes through 0.5 |x| |tanh'| <= 0.5 |x| and is covered by 6u |x| (1 + x^2 / 20)).
+    GELU-erf = 0.5 x (1 + erff(x / sqrt 2)): erff is within 2 ulp; with the three fp32 operations <= 5u |x|.
+    Mish = x tanh.approx(sp), sp = __logf(1 + __expf(x)) (sp = x beyond 15): __expf has relative error
+    (2 + floor(1.173 |x|)) 2^-23 (<= 20 2^-23 for |x| <= 15); 1 + e rounds (u); __logf is within 2^-21.41 absolute for
+    arguments in [0.5, 2] and 3 ulp elsewhere; a relative error d of the argument moves the log by d.  So
+    |sp~ - sp| <= (20 2^-23 + u) + 2^-21.41 + 3 2^-23 sp, and tanh' <= 1 carries that to tanh.  The result is
+    |x| (|sp~ - sp| + EPS_TANH + u)."""
+    x, ax = v.double(), v.double().abs()
+    if act == 0:
+        return bv.clone()
+    if act in (1, 2):
+        prop = 1.13 * bv
+        if act == 1:
+            return prop + ax * (0.5 * EPS_TANH + 6 * U32 * (1 + x * x / 20))
+        return prop + 5 * U32 * ax
+    sp = torch.nn.functional.softplus(x)
+    dsp = 21 * 2.0 ** -23 + 2.0 ** -21.41 + 3 * 2.0 ** -23 * sp
+    dsp = torch.where(x > 15, U32 * ax, dsp)
+    return 1.1 * bv + ax * (dsp + EPS_TANH + U32)
+
+
+def out_bound(ref: torch.Tensor, b: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """Add the output rounding: the kernel rounds its fp32 value (within b of ref) once, relative error u_out."""
+    mag = ref.double().abs() + b
+    if dtype == torch.bfloat16:
+        return b + U_BF16 * mag
+    if dtype in (torch.uint8, torch.float8_e4m3fn):
+        return b + U_E4M3 * mag + E4M3_SUB
+    return b + U32 * mag
+
+
+def attention_ref(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, kv_len=None):
+    """float64 softmax(q k^T) v per (batch, head) for [B, H, N, 64] inputs; also returns p |v| (the softmax-weighted
+    mean of |v|) for attention_bound.  Keys at or beyond kv_len[b] are masked."""
+    q, k, v = q.double(), k.double(), v.double()
+    s = q @ k.transpose(-1, -2)
+    if kv_len is not None:
+        n = k.shape[2]
+        m = torch.arange(n, device=k.device)[None] < kv_len.to(k.device)[:, None].long()
+        s = s.masked_fill(~m[:, None, None, :], float("-inf"))
+    p = torch.softmax(s, -1)
+    return p @ v, p @ v.abs(), (q.abs() @ k.abs().transpose(-1, -2)).masked_fill(p == 0, 0).amax(-1, keepdim=True)
+
+
+def attention_bound(o: torch.Tensor, pv: torch.Tensor, qk_abs: torch.Tensor, logit_max: float, tiles: int,
+                    out_dtype=torch.bfloat16) -> torch.Tensor:
+    """Bound on the flash-attention output, per element.
+
+    The kernel forms p_i = ex2.approx(s_i log2 e - m log2 e), sums the fp32 p_i into l, multiplies bf16(p_i) by v_i
+    and scales the result by 1 / l.  O = sum w_i v_i with weights w_i = p_i / l; perturbing each p_i by a relative
+    error d_i moves O by at most 2 max|d| sum w_i |v_i| (numerator and denominator), i.e. 2 d p|v|.  Sources of d:
+    bf16 rounding of p in the P V product (U_BF16); the S = Q K^T accumulation (2u 65 sum |q||k|, logits' error times
+    ln-scale 1); the fp32 argument s log2e - m log2e (3u |s| log2e, then ln 2 per unit of log2) plus ex2.approx
+    (EPS_EX2); the running-max rescale of o and l (one ex2.approx and one product per 128-key tile, applied to both o
+    and l but rounded separately: 2 (EPS_EX2 + u) per tile).  The P V accumulation adds 2u (N + 1) p|v| as in
+    gemm_acc_bound, 1 / l and the product 3u |O|, and the output rounding u_out |O|."""
+    d = U_BF16 + 2 * U32 * 65 * qk_abs + 3 * U32 * abs(logit_max) * 1.4427 * 0.6932 + EPS_EX2 \
+        + 2 * tiles * (EPS_EX2 + U32)
+    b = 2 * d * pv + 2 * U32 * (tiles * 128 + 1) * pv + 3 * U32 * o.abs()
+    return out_bound(o, b, out_dtype)

@@ -1,0 +1,164 @@
+"""CPU: the element-wise checkers of kernel_check.py accept a correct result and reject, naming the right tile, the
+mistakes kernels make; and every GEMM instantiation gemm.cu builds has a GPU test at each tile width that reaches it."""
+import re
+from pathlib import Path
+
+import pytest
+import torch
+
+from kernel_check import (U32, Guarded, assert_exact, assert_within, attention_bound, attention_ref, attn_tiles,
+                          gemm_acc_bound, gemm_tiles, out_bound, rope_bound, rope_ref)
+
+ROOT = Path(__file__).resolve().parent.parent
+
+
+def _operands(M=300, N=136, K=256, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    a = torch.randn(M, K, generator=g).bfloat16()
+    w = (torch.randn(N, K, generator=g) * K ** -0.5).bfloat16()
+    return a, w
+
+
+def _fp32_matmul(a, w):
+    return a.float() @ w.float().T
+
+
+def _check(got, a, w, bn=64):
+    ref = a.double() @ w.double().T
+    b = out_bound(ref, gemm_acc_bound(a, w), torch.float32)
+    return assert_within(got, ref, b, gemm_tiles(bn), "self-test")
+
+
+def test_accepts_fp32_matmul():
+    a, w = _operands()
+    assert _check(_fp32_matmul(a, w), a, w) <= 1.0
+
+
+def test_exact_accepts_integer_matmul_and_names_first_bad_element():
+    g = torch.Generator().manual_seed(1)
+    a = torch.randint(-8, 9, (300, 200), generator=g).bfloat16()
+    w = torch.randint(-8, 9, (136, 200), generator=g).bfloat16()
+    got = _fp32_matmul(a, w)
+    want = (a.double() @ w.double().T).float()
+    assert_exact(got, want, gemm_tiles(64), "exact")
+    want[want == 0] = -0.0                   # signed zeros compare equal
+    assert_exact(got, want, gemm_tiles(64), "exact")
+    got[200, 70] += 1
+    with pytest.raises(AssertionError, match=r"tile \(m 1, n 1\) row 200 col 70"):
+        assert_exact(got, want, gemm_tiles(64), "exact")
+    got[200, 70] -= 1
+    got[5, 3] = 2.0 ** -140                  # a denormal is not zero
+    want[5, 3] = 0.0
+    with pytest.raises(AssertionError, match=r"row 5 col 3"):
+        assert_exact(got, want, gemm_tiles(64), "exact")
+
+
+def test_rejects_dropped_k_block():
+    a, w = _operands()
+    got = _fp32_matmul(a, w)
+    r, c = slice(128, 256), slice(64, 128)
+    got[r, c] -= a[r, 64:128].float() @ w[c, 64:128].float().T
+    with pytest.raises(AssertionError, match=r"tile \(m 1, n 1\)"):
+        _check(got, a, w)
+
+
+def test_rejects_row_shift_in_tile_tail():
+    a, w = _operands()
+    got = _fp32_matmul(a, w)
+    got[299] = got[298]               # last tile holds rows 256..299
+    with pytest.raises(AssertionError, match=r"tile \(m 2, n \d\) row 299"):
+        _check(got, a, w)
+
+
+def test_rejects_swapped_columns():
+    a, w = _operands()
+    got = _fp32_matmul(a, w)
+    got[:, [70, 71]] = got[:, [71, 70]]
+    with pytest.raises(AssertionError, match=r"tile \(m \d, n 1\) row \d+ col 7[01]"):
+        _check(got, a, w)
+
+
+def test_rejects_rope_position_off_by_one():
+    from f5_tts_mlx_b200.dit import rope_table
+    a, w = _operands(M=300, N=192, K=128)
+    tab = rope_table(301)
+    pos = torch.arange(300)
+    x = a.double() @ w.double().T
+    bx = gemm_acc_bound(a, w) + U32 * x.abs()
+    ref, b = rope_ref(x, tab, pos, 128), rope_bound(x, bx, tab, pos, 128)
+    b = out_bound(ref, b, torch.float32)
+    good = rope_ref(_fp32_matmul(a, w).double(), tab, pos, 128).float()
+    assert_within(good, ref, b, gemm_tiles(64), "rope")
+    bad_pos = pos.clone()
+    bad_pos[128:256] += 1
+    bad = rope_ref(_fp32_matmul(a, w).double(), tab, bad_pos, 128).float()
+    with pytest.raises(AssertionError, match=r"tile \(m 1, n [01]\)"):
+        assert_within(bad, ref, b, gemm_tiles(64), "rope")
+
+
+def test_rejects_leaked_masked_key():
+    B, N, H = 2, 300, 2
+    g = torch.Generator().manual_seed(3)
+    q, k, v = [(torch.randn(B, H, N, 64, generator=g) * s).bfloat16().float() for s in (0.4, 0.4, 1.0)]
+    kv = torch.tensor([300, 200])
+    o, pv, qk = attention_ref(q, k, v, kv)
+    b = attention_bound(o, pv, qk, qk.max().item(), 3)
+    flat = lambda t: t.permute(0, 2, 1, 3).reshape(B * N, H * 64)
+    got = flat(o).bfloat16()
+    assert_within(got, flat(o), flat(b), attn_tiles(N), "attention")
+    leak, _, _ = attention_ref(q, k, v, torch.tensor([300, 201]))
+    bad = o.clone()
+    bad[1, 1, 128:256] = leak[1, 1, 128:256]
+    with pytest.raises(AssertionError, match=r"\(batch 1, head 1, q-tile 1\)"):
+        assert_within(flat(bad).bfloat16(), flat(o), flat(b), attn_tiles(N), "attention")
+
+
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.uint8])
+def test_guard_detects_overwrite_and_unwritten(dtype):
+    g = Guarded(10, 20, dtype, "cpu")
+    assert g.view.stride(0) > 20
+    g.view.zero_()
+    g.check("clean")
+    g.buf.view(torch.uint8)[0, 0] ^= 1       # one byte of the first guard row
+    with pytest.raises(AssertionError, match="guard element overwritten at buffer row -3"):
+        g.check("overwrite")
+    g2 = Guarded(10, 20, dtype, "cpu")
+    g2.view[:, :19].zero_()
+    with pytest.raises(AssertionError, match="never written; first at row 0 col 19"):
+        g2.check("unwritten")
+
+
+# ---------------------------------------------------------------- instantiation coverage
+_ACT = {"ACT_NONE": 0, "ACT_GELU_TANH": 1, "ACT_GELU_ERF": 2, "ACT_MISH": 3}
+_B = {"true": True, "false": False}
+
+
+def built_instantiations():
+    """(ACT, OUT_BF16, ROPE, FP8, RESID) of every launch_gemm instantiation dispatch_epi (gemm.cu) can reach."""
+    src = (ROOT / "f5_tts_mlx_b200" / "csrc" / "gemm.cu").read_text()
+    body = src[src.index("static int dispatch_epi"):]
+    body = body[:body.index("\n}\n")]
+    out = set()
+    for m in re.finditer(r"launch_gemm<BN, kStages, (ACT_\w+), (true|false), (true|false), (true|false), (true|false)>", body):
+        out.add((_ACT[m[1]], _B[m[2]], _B[m[3]], _B[m[4]], _B[m[5]]))
+    for m in re.finditer(r"^\s*F5_CASE(8?)\((ACT_\w+), (true|false), (true|false)\)", body, re.M):
+        out.add((_ACT[m[2]], _B[m[3]], _B[m[4]], m[1] == "8", True))
+    return out
+
+
+def test_dispatch_parse_sees_every_instantiation():
+    built = built_instantiations()
+    assert len(built) == 14, sorted(built)
+    assert (1, True, False, True, False) in built and (1, True, False, False, False) in built
+
+
+def test_every_instantiation_has_gpu_cases_at_each_tile_width():
+    import test_gpu_kernel_exact as ex
+    import test_gpu_kernels as kn
+    declared = set(ex.INSTANTIATIONS) | set(kn.INSTANTIATIONS)
+    built = built_instantiations()
+    # every declared case launches an instantiation that exists (the Python restatement of dispatch_epi is right)
+    assert {d[:5] for d in declared} <= built, sorted({d[:5] for d in declared} - built)
+    # every instantiation at both tile widths (only the grouped convolution is limited to 64, and none is grouped-only)
+    missing = sorted((i, bn) for i in built for bn in (64, 128) if i + (bn,) not in declared)
+    assert not missing, f"instantiations without a GPU case: {missing}"
