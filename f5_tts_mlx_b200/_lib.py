@@ -67,6 +67,8 @@ class GemmArgs(C.Structure):
         ("ln_scale", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_in_stats", C.c_void_p),
         ("ln_tab", C.c_void_p), ("ln_tab_ld", C.c_int64),
         ("ab_fp8", C.c_int32), ("out2_fp8", C.c_int32), ("acc_scale", C.c_float), ("out_fp8", C.c_int32),
+        ("a_scale", C.c_void_p), ("a_scale_ld", C.c_int64), ("w_scale", C.c_void_p), ("out_scale", C.c_void_p),
+        ("out2_scale", C.c_void_p),
     ]
 
 
@@ -101,6 +103,8 @@ SYMBOLS: dict[str, tuple] = {
                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "f5_attention_fwd_e4m3": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "f5_attention_fwd_e4m3_scaled": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
+                                               C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_ln_modulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]),
     "f5_dwconv7_ln": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,

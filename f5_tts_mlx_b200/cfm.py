@@ -332,9 +332,10 @@ class F5TTS:
         return out, trajectory
 
     @classmethod
-    def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None):
+    def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None):
+        """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8)."""
         from .pretrained import from_pretrained
-        return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits)
+        return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8)
 
 
 CFM = F5TTS

@@ -9,7 +9,8 @@ extern "C" int f5_debug_attention_ts(void* base) {
 }
 
 static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch, int32_t frames,
-                          int32_t heads, int32_t head_dim, const int32_t* kv_len, int out_fp8, void* stream_);
+                          int32_t heads, int32_t head_dim, const int32_t* kv_len, int out_fp8, void* stream_,
+                          float* scale_out = nullptr);
 
 extern "C" int f5_attention_fwd(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out,
                                 int32_t batch, int32_t frames, int32_t heads, int32_t head_dim,
@@ -22,9 +23,17 @@ extern "C" int f5_attention_fwd_e4m3(const void* qkv, int64_t ld_qkv, void* out,
                                      const int32_t* kv_len, void* stream_) {
   return attention_impl(qkv, ld_qkv, out, ld_out, batch, frames, heads, head_dim, kv_len, 1, stream_);
 }
+// block-scaled e4m3 output: each (row, head) with its own power-of-two scale, scale_out fp32 [heads][batch * frames]
+extern "C" int f5_attention_fwd_e4m3_scaled(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out,
+                                            int32_t batch, int32_t frames, int32_t heads, int32_t head_dim,
+                                            const int32_t* kv_len, float* scale_out, void* stream_) {
+  F5_REQUIRE(scale_out != nullptr, "f5_attention_fwd_e4m3_scaled: null scale_out");
+  return attention_impl(qkv, ld_qkv, out, ld_out, batch, frames, heads, head_dim, kv_len, 1, stream_, scale_out);
+}
 
 static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch, int32_t frames,
-                          int32_t heads, int32_t head_dim, const int32_t* kv_len, int out_fp8, void* stream_) {
+                          int32_t heads, int32_t head_dim, const int32_t* kv_len, int out_fp8, void* stream_,
+                          float* scale_out) {
   using namespace f5;
   if (int e = device_check()) return e;
   F5_REQUIRE(qkv && out, "f5_attention_fwd: null pointer");
@@ -43,6 +52,7 @@ static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
   p.out = reinterpret_cast<__nv_bfloat16*>(out);
   p.ldo = (int)ld_out;
   p.out_fp8 = out_fp8;
+  p.scale_out = scale_out;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfScope ps(PROF_ATTN, 4.0 * batch * heads * (double)frames * frames * 64.0,
                2.0 * batch * (double)frames * heads * 64.0 * 4.0, stream);
@@ -54,7 +64,8 @@ static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
     return 0;
   };
   const dim3 grid(cdiv(frames, 128), heads, batch);
-  static SmemAttrOnce o4, o8;
+  static SmemAttrOnce o4, o8, o8s;
+  if (scale_out != nullptr) return launch(attn_fwd_kernel<true, true>, o8s, grid, 384, AttnSmem::kTotal);
   if (out_fp8) return launch(attn_fwd_kernel<true>, o8, grid, 384, AttnSmem::kTotal);
   return launch(attn_fwd_kernel<false>, o4, grid, 384, AttnSmem::kTotal);
 }

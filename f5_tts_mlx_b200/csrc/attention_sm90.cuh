@@ -21,6 +21,7 @@ struct AttnParams {
   int ldo;
   unsigned long long* prof;  // in-graph timing slot (ptx.cuh prof_stamp_*), or null
   int out_fp8;             // `out` receives e4m3 bytes (ldo in bytes) — the A operand of an FP8-mode out-projection
+  float* scale_out;        // block-scaled e4m3 output: [H][B*N] power-of-two scale per (row, head), or null
 };
 
 struct AttnSmem {
@@ -33,7 +34,8 @@ struct AttnSmem {
   static constexpr int kTotal = kBar + kNumBars * 8 + 1024;   // + align slack
 };
 
-template <bool kOut8>     // e4m3 output (FP8 mode), its own instantiation
+// kOut8: e4m3 output (FP8 mode), its own instantiation; kScaled (with kOut8): block-scaled e4m3, one scale per (row, head)
+template <bool kOut8, bool kScaled = false>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -172,15 +174,32 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p)
       l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
     }
     const float inv[2] = {1.f / l_run[0], 1.f / l_run[1]};
+    // block-scaled output: the (row, head) amax of O / l over the 4 threads that hold the row (two shuffles, taken by
+    // every lane before any row is skipped), then the row's scale and its reciprocal
+    float qs[2] = {1.f, 1.f}, qinv[2] = {1.f, 1.f};
+    if constexpr (kScaled) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float amax = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c)
+          amax = fmax_nan(amax, fmax_nan(fabsf(o[4 * c + 2 * r] * inv[r]), fabsf(o[4 * c + 2 * r + 1] * inv[r])));
+        amax = fmax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
+        amax = fmax_nan(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
+        qs[r] = e4m3_block_scale(amax, qinv[r]);
+      }
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int n = q0 + wg * 64 + rw + 8 * r;
       if (n >= p.N) continue;
       const size_t row = (size_t)b * p.N + n;
+      if (kScaled && (lane & 3) == 0) p.scale_out[(size_t)h * p.B * p.N + row] = qs[r];
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
         const int col = h * 64 + 8 * c + 2 * (lane & 3);
-        const float v0 = o[4 * c + 2 * r] * inv[r], v1 = o[4 * c + 2 * r + 1] * inv[r];
+        float v0 = o[4 * c + 2 * r] * inv[r], v1 = o[4 * c + 2 * r + 1] * inv[r];
+        if constexpr (kScaled) { v0 *= qinv[r]; v1 *= qinv[r]; }
         if constexpr (kOut8) {
           uint16_t w;
           asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(w) : "f"(v1), "f"(v0));   // first source -> upper byte

@@ -16,6 +16,8 @@ extern "C" int f5_attention_fwd(const void*, int64_t, void*, int64_t, int32_t, i
                                 int32_t, const int32_t*, void*);
 extern "C" int f5_attention_fwd_e4m3(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
                                      int32_t, const int32_t*, void*);
+extern "C" int f5_attention_fwd_e4m3_scaled(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
+                                            int32_t, const int32_t*, float*, void*);
 
 namespace f5 {
 
@@ -176,6 +178,11 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
   static int fp8_level = -1;
   if (fp8_level < 0) { const char* v = getenv("F5_FP8_LEVEL"); fp8_level = (v && v[0] == '1') ? 1 : 2; }
   const bool fp8b = fp8 && fp8_level >= 2 && w->blocks[0].out_w8 != nullptr && w->blocks[0].ff2_w8 != nullptr;
+  // block-scaled FP8 (DESIGN.md section 8): per-channel weight scales and per-(row, 64-column unit) activation scales;
+  // all four block GEMMs run on e4m3 operands, whatever F5_FP8_LEVEL says
+  const f5_dit_block_weights& b0 = w->blocks[0];
+  const bool blk8 = fp8 && b0.out_w8 && b0.ff2_w8 && b0.qkv_ws && b0.ff1_ws && b0.out_ws && b0.ff2_ws &&
+                    b->a_fp8_scale && b->attn_scale && b->ff_scale;
   static const GemmTune t_qkv = tune_of("qkv"), t_out = tune_of("out"), t_ff1 = tune_of("ff1"), t_ff2 = tune_of("ff2");
   const long long tab_ld = ln_tab_ld(w);
   const float* tab = fused ? b->ln_tab + (size_t)4 * ti * tab_ld : nullptr;   // this time's 4 operand rows
@@ -206,6 +213,7 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
     if (fused) {   // the stream's first producer: operand + statistics for block 0's attn_norm
       g.ln_scale = (w->depth > 0 ? mod + D : mod + (size_t)w->depth * 6 * D); g.ln_stats = b->ln_stats;
       g.out2_bf16 = fp8 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = fp8 ? 1 : 0;
+      if (blk8) g.out2_scale = b->a_fp8_scale;
     }
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
@@ -221,16 +229,23 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       g.bias = bw.qkv_b;
       if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)l * (3 * D + F); g.ln_tab_ld = tab_ld; }
       if (fp8) { g.a = b->a_fp8; g.w = bw.qkv_w8; g.ab_fp8 = 1; g.acc_scale = bw.qkv_s8; }
+      if (blk8) { g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.qkv_ws; g.acc_scale = 1.f; }
       g.variant = t_qkv.variant; g.tile_n = t_qkv.tile_n;
       g.rows_per_batch = N; g.num_batches = BU;
       g.rope = b->rope; g.rope_cols = 2 * D; g.q_scale = 0.125f; g.q_cols = D;
       // weight prefetch chain (L2): while QKV runs, pull in out_w and ff1_w (contiguous in the pack)
       if (prefetch) { g.prefetch = bw.out_w; g.prefetch_bytes = (int64_t)2 * D * D; }
+      if (prefetch && blk8) { g.prefetch = bw.out_w8; g.prefetch_bytes = (int64_t)D * D; }   // the e4m3 weights it reads
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
-    if (int e = (fp8b ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
-                                                                  b->seq_len ? b->seq_len : b->valid_len, st))
+    if (blk8) {
+      if (int e = f5_attention_fwd_e4m3_scaled(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
+                                               b->seq_len ? b->seq_len : b->valid_len, b->attn_scale, st))
+        return e;
+    } else if (int e = (fp8b ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads,
+                                                                         64, b->seq_len ? b->seq_len : b->valid_len, st)) {
       return e;
+    }
     {
       f5_gemm_args g = gemm_base(b->c_bf16, D, bw.out_w, D, R, D, D, b->x, D, false);
       g.bias = bw.out_b;
@@ -243,6 +258,11 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
         g.out2_bf16 = fp8 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = fp8 ? 1 : 0;
       }
       if (fp8b) { g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = bw.out_s8; }     // A = c_bf16's bytes, e4m3 [R, D]
+      if (blk8) {
+        g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.out_ws;
+        g.a_scale = b->attn_scale; g.a_scale_ld = R; g.out2_scale = b->a_fp8_scale;
+        if (prefetch) { g.prefetch = bw.ff1_w8; g.prefetch_bytes = (int64_t)F * D; }
+      }
       g.variant = t_out.variant; g.tile_n = t_out.tile_n;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
@@ -256,6 +276,11 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       if (fp8b) g.out_fp8 = 1;                                                   // ff_bf16's bytes as e4m3 [R, F]
       g.variant = t_ff1.variant; g.tile_n = t_ff1.tile_n;
       if (prefetch) { g.prefetch = bw.ff2_w; g.prefetch_bytes = (int64_t)2 * D * F; }
+      if (blk8) {
+        g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.ff1_ws; g.acc_scale = 1.f;
+        g.out_fp8 = 1; g.out_scale = b->ff_scale;
+        if (prefetch) { g.prefetch = bw.ff2_w8; g.prefetch_bytes = (int64_t)D * F; }
+      }
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
     {
@@ -273,6 +298,13 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
         if (fp8 && l + 1 < w->depth) { g.out2_bf16 = b->a_fp8; g.out2_fp8 = 1; }   // proj_out (after the last block) stays bf16
       }
       if (fp8b) { g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff2_s8; }
+      if (blk8) {
+        g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.ff2_ws;
+        g.a_scale = b->ff_scale; g.a_scale_ld = R;
+        if (g.out2_fp8) g.out2_scale = b->a_fp8_scale;
+        g.prefetch = nullptr; g.prefetch_bytes = 0;
+        if (prefetch && l + 1 < w->depth) { g.prefetch = w->blocks[l + 1].qkv_w8; g.prefetch_bytes = (int64_t)3 * D * D; }
+      }
       g.variant = t_ff2.variant; g.tile_n = t_ff2.tile_n;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }

@@ -6,11 +6,11 @@
 
 namespace f5 {
 
-template <int BN, int kStages, int ACT, bool OUT_BF16, bool ROPE, bool FP8, bool RESID = true>
+template <int BN, int kStages, int ACT, bool OUT_BF16, bool ROPE, bool FP8, bool RESID = true, bool SCALED = false>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const CUtensorMap& to2,
                        const GemmParams& p, dim3 grid, cudaStream_t stream) {
-  using S = GemmSmem<BN, kStages>;
-  auto kern = gemm_bf16_tn_kernel<BN, kStages, ACT, OUT_BF16, ROPE, FP8, RESID>;
+  using S = GemmSmem<BN, kStages, SCALED>;
+  auto kern = gemm_bf16_tn_kernel<BN, kStages, ACT, OUT_BF16, ROPE, FP8, RESID, SCALED>;
   static SmemAttrOnce once;  // per instantiation
   F5_CHECK_CUDA(ensure_dyn_smem(once, kern, S::kTotal));
   const double taps = p.conv_taps;
@@ -56,6 +56,27 @@ static int dispatch_epi(int act, bool out_bf16, bool rope, const CUtensorMap& ta
 #undef F5_CASE
   return set_error(F5_ERR_INVALID, "f5_gemm_bf16: unsupported epilogue act=%d out_bf16=%d rope=%d",
                    act, (int)out_bf16, (int)rope);
+}
+
+// Block-scaled FP8 (any of a_scale / w_scale / out_scale / out2_scale set): only the epilogues of the DiT's block-scaled
+// mode are built — the RoPE QKV (bf16 out, no residual), the out-projection / FF2 (fp32 out, residual, scaled out2), FF1
+// (GELU, scaled e4m3 out, no residual) and the second conv-position GEMM (Mish, fp32 out, bf16 operands, scaled out2).
+// The bf16-output ones carry no residual tiles, which keeps their 128-wide instantiations free of spills.
+template <int BN, int kStages>
+static int dispatch_scaled(int act, bool out_bf16, bool rope, const CUtensorMap& ta, const CUtensorMap& tb,
+                           const CUtensorMap& to, const CUtensorMap& to2, const GemmParams& p, dim3 grid,
+                           cudaStream_t stream) {
+  const bool resid = p.resid != nullptr;
+  if (act == ACT_NONE && out_bf16 && rope && !resid)
+    return launch_gemm<BN, kStages, ACT_NONE, true, true, true, false, true>(ta, tb, to, to2, p, grid, stream);
+  if (act == ACT_NONE && !out_bf16 && !rope)
+    return launch_gemm<BN, kStages, ACT_NONE, false, false, true, true, true>(ta, tb, to, to2, p, grid, stream);
+  if (act == ACT_GELU_TANH && out_bf16 && !rope && !resid)
+    return launch_gemm<BN, kStages, ACT_GELU_TANH, true, false, true, false, true>(ta, tb, to, to2, p, grid, stream);
+  if (act == ACT_MISH && !out_bf16 && !rope)
+    return launch_gemm<BN, kStages, ACT_MISH, false, false, true, true, true>(ta, tb, to, to2, p, grid, stream);
+  return set_error(F5_ERR_INVALID, "f5_gemm_bf16: block-scaled FP8 is not built for epilogue act=%d out_bf16=%d rope=%d "
+                   "resid=%d", act, (int)out_bf16, (int)rope, (int)resid);
 }
 
 }  // namespace f5
@@ -116,6 +137,13 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
     F5_REQUIRE(a->ln_tab && a->ln_tab_ld >= a->n && !a->out2_bf16 && taps == 1 && a->k % 128 == 0,
                "f5_gemm_bf16: ln_in_stats needs ln_tab (ld >= n), no second output, a plain GEMM with k %% 128 == 0");
   }
+  const bool scaled = a->a_scale || a->w_scale || a->out_scale || a->out2_scale;
+  if (a->a_scale)
+    F5_REQUIRE(ab8 && a->a_scale_ld >= a->m, "f5_gemm_bf16: a_scale needs ab_fp8 and a_scale_ld >= m");
+  if (a->out_scale)
+    F5_REQUIRE(a->out_fp8 && a->n % 64 == 0, "f5_gemm_bf16: out_scale needs out_fp8 and n %% 64 == 0");
+  if (a->out2_scale)
+    F5_REQUIRE(a->out2_bf16 && a->out2_fp8 && a->n % 64 == 0, "f5_gemm_bf16: out2_scale needs an e4m3 out2 and n %% 64 == 0");
   if (a->resid) F5_REQUIRE(a->ldr % 4 == 0, "f5_gemm_bf16: ldr not multiple of 4");
   if (a->gate) F5_REQUIRE(a->gate_ld % 4 == 0, "f5_gemm_bf16: gate_ld not multiple of 4");
 
@@ -175,6 +203,8 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   p.ln_in_stats = reinterpret_cast<const float2*>(a->ln_in_stats); p.ln_in_units = a->k / 64;
   p.ln_tab = a->ln_tab; p.ln_tab_ld = a->ln_tab_ld;
   p.ab8 = ab8 ? 1 : 0; p.acc_scale = ab8 ? a->acc_scale : 1.f; p.out2_fp8 = a->out2_fp8; p.out_fp8 = a->out_fp8;
+  p.a_scale = a->a_scale; p.a_scale_ld = a->a_scale_ld; p.w_scale = a->w_scale;
+  p.out_scale = a->out_scale; p.out2_scale = a->out2_scale;
   if (a->out2_bf16) F5_REQUIRE(a->ldo2 % 8 == 0 && a->n % 8 == 0, "f5_gemm_bf16: out2 alignment");
 
   // A: (channels, frames, utterances); flat mode is one "utterance" of m rows
@@ -197,6 +227,10 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   dim3 grid(cdiv(a->n, bn), batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128), 1);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const bool rope = a->rope != nullptr;
+  if (scaled) {
+    if (bn == 128) return dispatch_scaled<128, 4>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
+    return dispatch_scaled<64, 6>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
+  }
   if (bn == 128) return dispatch_epi<128, 4>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
   return dispatch_epi<64, 6>(a->act, a->out_bf16 != 0, rope, ta, tb, to, to2, p, grid, stream);
 }

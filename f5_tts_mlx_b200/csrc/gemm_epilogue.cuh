@@ -54,6 +54,12 @@ struct GemmParams {
   float acc_scale;         // multiplies the accumulator (the weight tensor's quantisation scale); 1 otherwise
   int out2_fp8;            // the second output is e4m3 (1 byte per element) instead of bf16
   int out_fp8;             // the primary output is e4m3 (bf16-output instantiations only): 32-byte rows per chunk
+  // ---- block-scaled FP8 (SCALED instantiations only; DESIGN.md section 8): power-of-two scales, x ~= s * e4m3 ----
+  const float* a_scale;    // [K/64][a_scale_ld]: scale of A per (row, 64-column unit), or null (A unscaled)
+  long long a_scale_ld;
+  const float* w_scale;    // [N]: per-output-channel weight scale (multiplies acc_scale), or null
+  float* out_scale;        // [N/64][M]: with out_fp8, `out` is quantised per (row, 64-column unit) and the scales written
+  float* out2_scale;       // [N/64][M]: the same for out2 (out2_fp8)
 };
 
 // Each CTA touches its 1/num_ctas slice of [pf_ptr, pf_ptr + pf_bytes) with L2 prefetches (one warp,
@@ -106,13 +112,15 @@ __device__ __forceinline__ float mish_fast(float x) {
 // gate_ld == 0) into shared memory; called by the 128 epilogue threads, `et` = 0..127
 // aux_s: c1 of the fused-LN consumer mode, or the second output's scale 1 + ln_scale (1 when there is none) — a GEMM is
 // never both.  In consumer mode bias_s holds c2 + bias.
-template <int BN>
+// ws_s (SCALED instantiations): acc_scale * w_scale[col], the factor of the accumulator term.
+template <int BN, bool SC = false>
 __device__ __forceinline__ void epi_stage_cols(const GemmParams& p, int n0, int et, float* bias_s,
-                                               float* gate_s, float* aux_s) {
+                                               float* gate_s, float* aux_s, float* ws_s = nullptr) {
 #pragma unroll
   for (int i = et; i < BN; i += 128) {
     const int col = n0 + i;
     const bool ok = col < p.N;
+    if constexpr (SC) ws_s[i] = (p.w_scale != nullptr && ok) ? p.acc_scale * p.w_scale[col] : p.acc_scale;
     float b = (p.bias != nullptr && ok) ? p.bias[col] : 0.f;
     float x = (p.ln_scale != nullptr && ok) ? 1.f + p.ln_scale[col] : 1.f;
     if (p.ln_in_stats != nullptr && ok) {
@@ -252,19 +260,118 @@ __device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiSta
   }
 }
 
+// Block-scaled e4m3 output of one 64-column unit (the unit's scale needs both chunks, so it is quantised and stored once
+// chunk B is done).  Chunk A is not held in registers: its fp32 values wait in the fp32 staging buffer of chunk A
+// (epi_store_tma's 128-byte SWIZZLE_128B rows at st.buf), written there by HALF 0 — as the staged fp32 `out` store of
+// the producer form, or, for the e4m3 primary output, by this thread alone (its own row: no barrier) — and are read
+// back by the same thread in HALF 1.
+__device__ __forceinline__ void epi_stage_f32(uint8_t* buf, int r, const float (&v)[32]) {
+  uint8_t* mine = buf + r * 128;
+  const int sw = r & 7;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    *reinterpret_cast<float4*>(mine + ((j ^ sw) * 16)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+}
+
+// e4m3 codes of 32 values x = v * aux (aux = null: x = v), quantised as x * inv (inv = 1 / scale, exact)
+__device__ __forceinline__ void epi_quant32(const float (&v)[32], const float* aux, float inv, uint4 (&q)[2]) {
+  uint32_t w[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    float x[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) x[k] = (aux != nullptr ? v[4 * i + k] * aux[4 * i + k] : v[4 * i + k]) * inv;
+    w[i] = pack_e4m3x4(x[0], x[1], x[2], x[3]);
+  }
+  q[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  q[1] = make_uint4(w[4], w[5], w[6], w[7]);
+}
+
+// the same for chunk A, read back from this thread's row of the fp32 staging buffer
+__device__ __forceinline__ void epi_quant32_staged(const uint8_t* buf, int r, const float* aux, float inv, uint4 (&q)[2]) {
+  const uint8_t* mine = buf + r * 128;
+  const int sw = r & 7;
+  uint32_t w[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 a = *reinterpret_cast<const float4*>(mine + ((i ^ sw) * 16));
+    float x[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) x[k] = (aux != nullptr ? x[k] * aux[4 * i + k] : x[k]) * inv;
+    w[i] = pack_e4m3x4(x[0], x[1], x[2], x[3]);
+  }
+  q[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  q[1] = make_uint4(w[4], w[5], w[6], w[7]);
+}
+
+// HALF 1 of a block-scaled unit: the unit's scale from the running amax (NaN propagates), written to
+// scale[colA / 64][row] (rows past the matrix write none); then the e4m3 chunks A (colA) and B (colA + 32) are staged as
+// 32-byte rows (SWIZZLE_32B), 4 KB each — of `out` (OUT_BF16: the e4m3 primary output, in the second 16 KB of st.buf,
+// chunk A's fp32 values being in the first) or of out2 (in st.buf2, with the fp32 chunk B of `out` staged as in
+// epi_store_tma) — and stored.  Each staged piece is written as soon as it is formed, so that few values are live at once.
+template <bool OUT_BF16>
+__device__ __forceinline__ void epi_finish_unit8(const float (&v)[32], const float* aux, float amax, float* scale,
+                                                 int M, int colA, int row, bool row_ok, const EpiStage& st) {
+  float inv;
+  const float s = e4m3_block_scale(amax, inv);
+  if (row_ok) scale[(size_t)(colA >> 6) * M + row] = s;
+  uint8_t* q8 = OUT_BF16 ? st.buf + 16384 : st.buf2;
+  const int sw = (st.r >> 2) & 1;
+  {
+    uint4 q[2];
+    epi_quant32(v, aux, inv, q);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) *reinterpret_cast<uint4*>(q8 + 4096 + st.r * 32 + ((j ^ sw) * 16)) = q[j];
+  }
+  uint8_t* buf = st.buf + (st.par_base ^ 1) * 16384;
+  if constexpr (!OUT_BF16) epi_stage_f32(buf, st.r, v);
+  {
+    uint4 q[2];
+    epi_quant32_staged(st.buf + st.par_base * 16384, st.r, aux != nullptr ? aux - 32 : nullptr, inv, q);
+#pragma unroll
+    for (int j = 0; j < 2; ++j) *reinterpret_cast<uint4*>(q8 + st.r * 32 + ((j ^ sw) * 16)) = q[j];
+  }
+  fence_proxy_async_smem();
+  if (st.et == 0) tma_store_wait_read<0>();
+  asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
+  if (st.et == 0) {
+    if constexpr (!OUT_BF16) tma_store_3d(st.map_out, buf, colA + 32, st.c1, st.c2);
+    const CUtensorMap* m8 = OUT_BF16 ? st.map_out : st.map_out2;
+    tma_store_3d(m8, q8, colA, st.c1, st.c2);
+    tma_store_3d(m8, q8 + 4096, colA + 32, st.c1, st.c2);
+    tma_store_commit();
+  }
+}
+
 // HALF: which 32-column half of a 64-column head this chunk is (static RoPE register indexing)
 // `unit_acc`: running (sum, sum of squares) of this thread's row over the 64-column unit (HALF 0 starts it, HALF 1
 // completes and stores it) — fused-LN producer mode only.
-template <int ACT, bool OUT_BF16, bool ROPE, int HALF>
+// SC (block-scaled instantiations): the accumulator term is multiplied by ws_s[col] (acc_scale * w_scale); a block-scaled
+// e4m3 output carries the running amax of its 64-column unit from chunk A to chunk B in `unit_amax`.
+template <int ACT, bool OUT_BF16, bool ROPE, int HALF, bool SC = false>
 __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float4 (&res)[8],
                                           const float* bias_s, const float* gate_s, const float* aux_s,
                                           const float2 (&cs)[ROPE ? 32 : 1], const GemmParams& p,
                                           int col0, int row, int b_idx, bool row_ok, bool row_valid,
-                                          const EpiStage& st, float2& unit_acc) {
+                                          const EpiStage& st, float2& unit_acc, const float* ws_s = nullptr,
+                                          float* unit_amax = nullptr) {
   float v[32];
   // rstd * acc - (mean * rstd) * c1 + (c2 + bias): the fused-LN consumer; (mu_r, rstd) = (0, 1) otherwise.
   // acc_scale (the e4m3 weight tensor's scale in FP8 mode, else 1) belongs to the accumulator term only.
-  if (p.ln_in_stats != nullptr) {          // uniform: only a fused-LN consumer pays for the mean term
+  if constexpr (SC) {
+    // rstd * w_s[col] * acc - mu_r * c1 + c2 for the fused-LN consumer, and acc * w_s[col] + bias otherwise: with
+    // (mu_r, rstd) = (0, 1) the same expression (rstd * w_s = w_s and -0 * aux + bias = bias exactly; aux is 1 + s or 1)
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+      const float4 bb = *reinterpret_cast<const float4*>(bias_s + j);
+      const float4 cc = *reinterpret_cast<const float4*>(aux_s + j);
+      const float4 ww = *reinterpret_cast<const float4*>(ws_s + j);
+      v[j] = fmaf(__uint_as_float(acc[j]), st.rstd * ww.x, fmaf(-st.mu_r, cc.x, bb.x));
+      v[j + 1] = fmaf(__uint_as_float(acc[j + 1]), st.rstd * ww.y, fmaf(-st.mu_r, cc.y, bb.y));
+      v[j + 2] = fmaf(__uint_as_float(acc[j + 2]), st.rstd * ww.z, fmaf(-st.mu_r, cc.z, bb.z));
+      v[j + 3] = fmaf(__uint_as_float(acc[j + 3]), st.rstd * ww.w, fmaf(-st.mu_r, cc.w, bb.w));
+    }
+  } else if (p.ln_in_stats != nullptr) {   // uniform: only a fused-LN consumer pays for the mean term
     const float ra = st.rstd * p.acc_scale;
 #pragma unroll
     for (int j = 0; j < 32; j += 4) {
@@ -350,6 +457,20 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
         unit_acc = make_float2((s1[0] + s1[1]) + (s1[2] + s1[3]), (s2[0] + s2[1]) + (s2[2] + s2[3]));
         if (HALF == 1 && row_ok && col0 < p.N) p.ln_stats[(size_t)row * (p.N >> 6) + (col0 >> 6)] = unit_acc;
       }
+      if constexpr (SC) {
+        if (p.out2_fp8 && p.out2_scale != nullptr) {   // block-scaled e4m3 operand x (1 + s): one scale per unit
+          float amax = HALF == 0 ? 0.f : *unit_amax;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) amax = fmax_nan(amax, fabsf(v[j] * aux_s[j]));
+          if (HALF == 0) {
+            *unit_amax = amax;
+            epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0);    // the fp32 chunk A leaves now (and stays staged)
+          } else {
+            epi_finish_unit8<OUT_BF16>(v, aux_s, amax, p.out2_scale, p.M, col0 - 32, row, row_ok, st);
+          }
+          return;
+        }
+      }
       uint4 w2[4];
       if (p.out2_fp8) {      // e4m3 operand of an FP8-mode consumer: 32 bytes per row and chunk
 #pragma unroll
@@ -376,6 +497,20 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
       return;
     }
   }
+  if constexpr (SC && OUT_BF16) {
+    if (st.out_fp8 && p.out_scale != nullptr) {   // block-scaled e4m3 output (FF1's GELU output)
+      float amax = HALF == 0 ? 0.f : *unit_amax;
+#pragma unroll
+      for (int j = 0; j < 32; ++j) amax = fmax_nan(amax, fabsf(v[j]));
+      if (HALF == 0) {
+        *unit_amax = amax;
+        epi_stage_f32(st.buf + st.par_base * 16384, st.r, v);   // chunk A waits in its (own-row) fp32 staging
+      } else {
+        epi_finish_unit8<OUT_BF16>(v, nullptr, amax, p.out_scale, p.M, col0 - 32, row, row_ok, st);
+      }
+      return;
+    }
+  }
   epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0);   // all 128 threads of the group take part (barrier inside)
 }
 
@@ -391,13 +526,15 @@ __device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&acc)[32]) 
 
 // Drains one accumulator tile of BN columns: `acc_row` = this thread's row of the shared-memory accumulator tile,
 // already offset to the group's first column.  `res0` holds the residual of the first 32 columns.
-template <int BN, int ACT, bool OUT_BF16, bool ROPE>
+template <int BN, int ACT, bool OUT_BF16, bool ROPE, bool SC = false>
 __device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float* bias_s,
                                                const float* gate_s, const float* aux_s, const float2 (&cs)[ROPE ? 32 : 1],
                                                float4 (&res0)[8], const GemmParams& p, int n0, int row,
-                                               int b_idx, bool row_ok, bool row_valid, EpiStage& st) {
+                                               int b_idx, bool row_ok, bool row_valid, EpiStage& st,
+                                               const float* ws_s = nullptr) {
   float4 res1[8];
   float2 unit_acc = make_float2(0.f, 0.f);
+  float unit_amax = 0.f;
   st.par_base = 0;
 #pragma unroll 1
   for (int cc = 0; cc < BN / 64; ++cc) {
@@ -407,14 +544,16 @@ __device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float
     epi_load_resid(p, row, colB, row_ok, res1);
     acc_ld32(acc_row + cc * 64, acc);
     if (colA < p.N)   // uniform per CTA
-      epi_apply<ACT, OUT_BF16, ROPE, 0>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
-                                        b_idx, row_ok, row_valid, st, unit_acc);
+      epi_apply<ACT, OUT_BF16, ROPE, 0, SC>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
+                                            b_idx, row_ok, row_valid, st, unit_acc, SC ? ws_s + cc * 64 : nullptr,
+                                            &unit_amax);
     // chunk B: request the next unit's first residual, then drain B
     if (cc + 1 < BN / 64) epi_load_resid(p, row, colA + 64, row_ok, res0);
     acc_ld32(acc_row + cc * 64 + 32, acc);
     if (colB < p.N)
-      epi_apply<ACT, OUT_BF16, ROPE, 1>(acc, res1, bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs, p,
-                                        colB, row, b_idx, row_ok, row_valid, st, unit_acc);
+      epi_apply<ACT, OUT_BF16, ROPE, 1, SC>(acc, res1, bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs,
+                                            p, colB, row, b_idx, row_ok, row_valid, st, unit_acc,
+                                            SC ? ws_s + cc * 64 + 32 : nullptr, &unit_amax);
   }
 }
 

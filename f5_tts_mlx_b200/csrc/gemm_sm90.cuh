@@ -31,7 +31,7 @@
 
 namespace f5 {
 
-template <int BN, int kStages>
+template <int BN, int kStages, bool SCALED = false>
 struct GemmSmem {
   static constexpr int kABytes = 128 * 128;           // 128 rows x 128 bytes (64 bf16 / 128 e4m3)
   static constexpr int kBBytes = BN * 128;
@@ -40,7 +40,8 @@ struct GemmSmem {
   static constexpr int kAccLd = BN + 4;                // floats per accumulator row: conflict-free row-wise float4 reads
   static constexpr int kBarOffset = kAccOffset + 128 * kAccLd * 4;
   static constexpr int kColsOffset = (kBarOffset + 2 * kStages * 8 + 15) & ~15;   // bias_s[BN], gate_s[BN], aux_s[BN]
-  static constexpr int kTotal = kColsOffset + 3 * BN * 4 + 1024;  // + align slack
+  // block-scaled instantiations also stage ws_s[BN] (the per-column weight scale)
+  static constexpr int kTotal = kColsOffset + (SCALED ? 4 : 3) * BN * 4 + 1024;  // + align slack
   // epilogue store staging reuses the (idle) operand ring: fp32/bf16 chunks at [0, 64 KB) (32 KB per group), the
   // bf16 copy of the fused-LN producer mode at [64 KB, 96 KB) (16 KB per group, two alternating 8 KB buffers)
   static_assert(kStages * kStageBytes >= 98304, "operand ring too small for the epilogue staging");
@@ -70,7 +71,10 @@ __device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t da, ui
 // FP8 = false instantiations have every e4m3 feature (ab8 / out_fp8 / out2_fp8 / acc_scale) folded away at compile
 // time, so only the FP8 mode pays for the FP8 mode.  RESID = false instantiations (no residual input) drop the
 // residual tiles from the epilogue's registers.
-template <int BN, int kStages, int ACT, bool OUT_BF16, bool ROPE, bool FP8 = false, bool RESID = true>
+// SCALED = true (block-scaled FP8, DESIGN.md section 8): A may carry a power-of-two scale per (row, 64-column unit), which
+// the main loop applies when it promotes each unit's e4m3 wgmma partial; the epilogue multiplies the accumulator by a
+// per-column weight scale and writes e4m3 outputs with one scale per (row, 64-column unit).
+template <int BN, int kStages, int ACT, bool OUT_BF16, bool ROPE, bool FP8 = false, bool RESID = true, bool SCALED = false>
 __global__ void __launch_bounds__(384, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
                     const __grid_constant__ CUtensorMap tma_b, const __grid_constant__ CUtensorMap tma_out,
@@ -78,7 +82,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
   GemmParams p = p_arg;
   if constexpr (!FP8) { p.ab8 = 0; p.out_fp8 = 0; p.out2_fp8 = 0; p.acc_scale = 1.f; }
   if constexpr (!RESID) p.resid = nullptr;
-  using S = GemmSmem<BN, kStages>;
+  if constexpr (!SCALED) { p.a_scale = nullptr; p.w_scale = nullptr; p.out_scale = nullptr; p.out2_scale = nullptr; }
+  using S = GemmSmem<BN, kStages, SCALED>;
   using E = GemmEpi<BN>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must sit on 1024-byte boundaries
@@ -172,7 +177,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
     float* bias_s = reinterpret_cast<float*>(smem + S::kColsOffset) + grp * BNG;
     float* gate_s = reinterpret_cast<float*>(smem + S::kColsOffset) + BN + grp * BNG;
     float* aux_s = reinterpret_cast<float*>(smem + S::kColsOffset) + 2 * BN + grp * BNG;
-    if (grp < E::kGroups) epi_stage_cols<BNG>(p, n0g, et, bias_s, gate_s, aux_s);   // under the main loop's loads
+    float* ws_s = SCALED ? reinterpret_cast<float*>(smem + S::kColsOffset) + 3 * BN + grp * BNG : nullptr;
+    if (grp < E::kGroups) epi_stage_cols<BNG, SCALED>(p, n0g, et, bias_s, gate_s, aux_s, ws_s);   // under the main loop's loads
 
     float acc[BN / 2];
 #pragma unroll
@@ -222,8 +228,55 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
         wgmma_reg_fence(acc);
       }
     };
-    if (p.ab8) mma_loop(std::true_type{});
-    else mma_loop(std::false_type{});
+    // Block-scaled A: each 128-byte e4m3 k-block holds two 64-element units with their own row scales.  A unit's two
+    // k32 wgmmas go to a fresh partial that is promoted as acc = fma(part, s_a[row], acc).  The thread's fragment rows
+    // are r and r + 8 (acc[i] belongs to row r + 8 ((i / 2) % 2)); their scales are loaded before the stage's wait,
+    // and only for rows that exist (TMA zero-fills A past the matrix or the utterance, a plain load would not).
+    auto mma_loop_scaled = [&]() {
+      const uint32_t ring = smem_u32(smem);
+      int s = 0;
+      uint32_t ph = 0;
+      const int t0 = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+      const int lim = p.tiles_per_batch > 0 ? p.rows_per_batch - m_in_batch0 : p.M - row0;   // rows of the tile that exist
+      const bool ok0 = t0 < lim, ok1 = t0 + 8 < lim;
+      const float* sp = p.a_scale + row0 + t0;
+      const size_t ld = (size_t)p.a_scale_ld;
+      float part[BN / 2];
+      for (int kb = 0; kb < num_kb; ++kb) {
+        float sc[2][2];   // [unit][row]
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const float* su = sp + (size_t)(2 * kb + u) * ld;
+          sc[u][0] = ok0 ? su[0] : 0.f;
+          sc[u][1] = ok1 ? su[8] : 0.f;
+        }
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = ring + s * S::kStageBytes + wg * (64 * 128), sb = ring + s * S::kStageBytes + S::kABytes;
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 2; ++k)
+            gemm_wgmma<BN, true>(part, gmma_desc_sw128(sa + 64 * u + 32 * k, 16, 1024),
+                                 gmma_desc_sw128(sb + 64 * u + 32 * k, 16, 1024), k != 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_reg_fence(part);
+          if (u == 1) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = fmaf(part[i], sc[u][(i >> 1) & 1], acc[i]);
+        }
+        if (++s == kStages) { s = 0; ph ^= 1; }
+      }
+    };
+    if constexpr (SCALED) {
+      if (p.ab8 && p.a_scale != nullptr) mma_loop_scaled();
+      else if (p.ab8) mma_loop(std::true_type{});
+      else mma_loop(std::false_type{});
+    } else {
+      if (p.ab8) mma_loop(std::true_type{});
+      else mma_loop(std::false_type{});
+    }
 
     // accumulator fragments -> fp32 tile in shared memory (row-major, kAccLd floats per row)
     {
@@ -280,8 +333,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
       stg.buf2_par = 8192;
       stg.mu_r = ln_mu_r; stg.rstd = ln_rstd;
       stg.out_fp8 = p.out_fp8;
-      epi_drain_tile<BNG, ACT, OUT_BF16, ROPE>(acc_s + r_in_tile * S::kAccLd + grp * BNG, bias_s, gate_s, aux_s, cs,
-                                               res0, p, n0g, row, b_idx, row_ok, row_valid, stg);
+      epi_drain_tile<BNG, ACT, OUT_BF16, ROPE, SCALED>(acc_s + r_in_tile * S::kAccLd + grp * BNG, bias_s, gate_s, aux_s,
+                                                       cs, res0, p, n0g, row, b_idx, row_ok, row_valid, stg, ws_s);
       if (et == 0) tma_store_wait_read<0>();   // the staging buffers must outlive the TMA unit's reads; grid completion
                                                // makes the global writes visible to the dependent kernel
     }

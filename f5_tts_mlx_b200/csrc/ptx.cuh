@@ -280,4 +280,26 @@ __device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float
   return (uint32_t)lo | ((uint32_t)hi << 16);
 }
 
+// max that propagates NaN (fmaxf drops it): the amax of a block-scaled unit that holds a NaN is NaN, as on the host
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float y;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(y) : "f"(a), "f"(b));
+  return y;
+}
+
+// Block-scaled FP8 (DESIGN.md section 8): the scale of a block with largest magnitude `amax` (>= 0) is the smallest power
+// of two s >= 2^-126 with amax <= 448 s, read off amax's exponent and mantissa bits (1.75 = 448 / 2^8 is mantissa
+// 0x600000), so that the scale, and x * (1 / s), are exact and equal to the host rule (weights.e4m3_block_scale).
+// amax == 0 gives 1; a non-finite amax is returned as the scale (1 / s = 0), so the block dequantises non-finite.
+__device__ __forceinline__ float e4m3_block_scale(float amax, float& inv) {
+  const uint32_t b = __float_as_uint(amax);
+  const int e = (int)(b >> 23) & 0xFF;
+  if (e == 0xFF) { inv = 0.f; return amax; }
+  if (b == 0u) { inv = 1.f; return 1.f; }
+  int k = e - 135 + ((b & 0x7FFFFFu) > 0x600000u ? 1 : 0);
+  k = k < -126 ? -126 : k;
+  inv = __uint_as_float((uint32_t)(127 - k) << 23);
+  return __uint_as_float((uint32_t)(k + 127) << 23);
+}
+
 }  // namespace f5

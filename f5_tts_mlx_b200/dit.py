@@ -12,7 +12,7 @@ from typing import Dict, Optional
 import torch
 
 from . import _lib
-from .weights import DiTConfig, PackedDiT, Weights
+from .weights import FP8_SCALINGS, DiTConfig, PackedDiT, Weights
 
 
 class DitBuffersC(C.Structure):
@@ -28,6 +28,7 @@ class DitBuffersC(C.Structure):
         ("c_bf16", C.c_void_p), ("qkv_bf16", C.c_void_p), ("ff_bf16", C.c_void_p), ("v", C.c_void_p),
         ("ln_stats", C.c_void_p), ("ln_tab", C.c_void_p), ("ln_prep", C.c_void_p),
         ("valid_len", C.c_void_p), ("a_fp8", C.c_void_p),
+        ("a_fp8_scale", C.c_void_p), ("attn_scale", C.c_void_p), ("ff_scale", C.c_void_p),
     ]
 
 
@@ -46,7 +47,8 @@ class DitSession:
     evaluation times, with or without the CFG batch doubling."""
 
     def __init__(self, cfg: DiTConfig, ct_ld: int, batch: int, frames: int, n_times: int, use_cfg: bool,
-                 text_cols: int, device: torch.device, masked: bool, fused_adaln: bool = True, fp8: bool = False):
+                 text_cols: int, device: torch.device, masked: bool, fused_adaln: bool = True, fp8: bool = False,
+                 fp8_block: bool = False):
         self.cfg, self.batch, self.frames, self.n_times, self.use_cfg = cfg, batch, frames, n_times, use_cfg
         self.device = device
         D, F, Ct = cfg.dim, cfg.ff_inner, cfg.text_dim
@@ -88,6 +90,12 @@ class DitSession:
         self.ln_tab = z(4 * n_times, self.ln_tab_ld) if fused_adaln else None
         self.ln_prep = z(2 * cfg.depth + 1, 4 * n_times, D, dt=bf16) if fused_adaln else None
         self.a_fp8 = z(R, D, dt=torch.uint8) if (fp8 and fused_adaln) else None   # e4m3 operand of the QKV / FF1 GEMMs
+        # block-scaled FP8: power-of-two scales per (row, 64-column unit), unit-major, of a_fp8, of the attention output
+        # (e4m3 in c_bf16) and of the FF1 output (e4m3 in ff_bf16)
+        blk = fp8 and fp8_block and fused_adaln
+        self.a_fp8_scale = z(D // 64, R) if blk else None
+        self.attn_scale = z(cfg.heads, R) if blk else None
+        self.ff_scale = z(F // 64, R) if blk else None
         c = DitBuffersC()
         c.batch, c.frames, c.cfg, c.n_times = batch, frames, int(use_cfg), n_times
         c.text_len_max, c.drop_flags = self.text.shape[1], 0
@@ -141,7 +149,8 @@ class DiT:
 
     def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.0, ff_mult=4, mel_dim=100,
                  text_num_embeds=256, text_dim=None, text_mask_padding=True, conv_layers=0,
-                 device: str | torch.device = "cuda", fused_adaln: bool = True, fp8: bool = False):
+                 device: str | torch.device = "cuda", fused_adaln: bool = True, fp8: bool = False,
+                 fp8_scaling: str = "tensor"):
         if text_dim is None:
             text_dim = mel_dim
         if dim_head != 64 or dim != heads * dim_head:
@@ -166,6 +175,13 @@ class DiT:
         self.fp8 = bool(fp8)
         if self.fp8 and not self.fused_adaln:
             raise ValueError("fp8=True needs fused_adaln=True (the e4m3 operand is written by the GEMM epilogues)")
+        # fp8_scaling="block": per-output-channel power-of-two weight scales and a power-of-two scale per (row, 64
+        # columns) of every e4m3 activation, so that outlier channels and a residual stream beyond 448 keep their
+        # precision; all four block GEMMs run on e4m3 (DESIGN.md section 8).  "tensor": one scale per weight tensor.
+        if fp8_scaling not in FP8_SCALINGS:
+            raise ValueError(f"fp8_scaling must be one of {FP8_SCALINGS}, not {fp8_scaling!r}")
+        self.fp8_scaling = fp8_scaling
+        self.fp8_block = self.fp8 and fp8_scaling == "block"
         self.device = torch.device(device)
         self.packed: Optional[PackedDiT] = None
         self._sessions: Dict[tuple, DitSession] = {}
@@ -178,12 +194,12 @@ class DiT:
         W = dict(weights)
         if not any(k.startswith("transformer.") for k in W):
             W = {"transformer." + k: v for k, v in W.items()}
-        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8).load(W)
+        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8, fp8_scaling=self.fp8_scaling).load(W)
         return self
 
     def allocate_weights(self) -> "DiT":
         """Allocate the packed buffer without filling it (non-source ranks before the broadcast)."""
-        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8)
+        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8, fp8_scaling=self.fp8_scaling)
         return self
 
     def _require_weights(self) -> PackedDiT:
@@ -194,13 +210,13 @@ class DiT:
     # -- sessions --
     def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int,
                 masked: bool, bucketed: bool = False) -> DitSession:
-        key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8)
+        key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8, self.fp8_block)
         s = self._sessions.pop(key, None)
         if s is None:
             while len(self._sessions) >= self.session_cache_size:
                 self._sessions.pop(next(iter(self._sessions)))
             s = DitSession(self.config, self._require_weights().ct_ld, batch, frames, n_times, use_cfg,
-                           text_cols, self.device, masked, self.fused_adaln, self.fp8)
+                           text_cols, self.device, masked, self.fused_adaln, self.fp8, self.fp8_block)
             if bucketed:
                 s.use_bucketing()
         self._sessions[key] = s          # LRU order: most recently used last

@@ -67,8 +67,13 @@ def gemm(
     w_static: bool = False,                    # w is not written by the preceding kernel: its first tiles load before the PDL wait
     prefetch: torch.Tensor | None = None,      # weights of a later GEMM to pull into L2 while this one runs
     prefetch_bytes: int = 0,
+    a_scale: torch.Tensor | None = None,      # f32 [k/64, >=rows] block scales of a (row stride = a_scale_ld)
+    w_scale: torch.Tensor | None = None,      # f32 [n] per-output-channel weight scales
+    out_scale: torch.Tensor | None = None,    # f32 [n/64, rows] written with a block-scaled e4m3 out (out_fp8)
+    out2_scale: torch.Tensor | None = None,   # f32 [n/64, rows] written with a block-scaled e4m3 out2 (out2_fp8)
 ) -> torch.Tensor:
-    _need_cuda(a, w, out, bias, resid, gate, row_len, rope, out2, ln_scale, ln_stats, ln_in_stats, ln_tab, prefetch)
+    _need_cuda(a, w, out, bias, resid, gate, row_len, rope, out2, ln_scale, ln_stats, ln_in_stats, ln_tab, prefetch,
+               a_scale, w_scale, out_scale, out2_scale)
     if ab_fp8:
         a = a.view(torch.uint8) if a.dtype != torch.uint8 else a
         w = w.view(torch.uint8) if w.dtype != torch.uint8 else w
@@ -123,5 +128,17 @@ def gemm(
     if ln_in_stats is not None:
         assert ln_in_stats.dtype == torch.float32 and ln_tab is not None and ln_tab.dtype == torch.float32
         g.ln_in_stats, g.ln_tab, g.ln_tab_ld = ln_in_stats.data_ptr(), ln_tab.data_ptr(), ln_tab.stride(0)
+    for t in (a_scale, w_scale, out_scale, out2_scale):
+        assert t is None or (t.dtype == torch.float32 and t.stride(-1) == 1)
+    if a_scale is not None:
+        g.a_scale, g.a_scale_ld = a_scale.data_ptr(), a_scale.stride(0)
+    if w_scale is not None:
+        g.w_scale = w_scale.data_ptr()
+    if out_scale is not None:
+        assert out_scale.is_contiguous() and out_scale.shape[-1] == m
+        g.out_scale = out_scale.data_ptr()
+    if out2_scale is not None:
+        assert out2_scale.is_contiguous() and out2_scale.shape[-1] == m
+        g.out2_scale = out2_scale.data_ptr()
     _lib.check(_lib.load().f5_gemm_bf16(C.byref(g), _stream()))
     return out

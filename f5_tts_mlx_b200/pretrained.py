@@ -23,7 +23,7 @@ import torch
 from .dit import DiT
 from .parallel import load_weights_distributed
 from .vocos import Vocos
-from .weights import (BASE_CONFIG, VocosConfig, Weights, convert_upstream_keys, dequantize_mlx_checkpoint,
+from .weights import (BASE_CONFIG, FP8_SCALINGS, VocosConfig, Weights, convert_upstream_keys, dequantize_mlx_checkpoint,
                       random_dit_weights, random_vocos_weights)
 
 VOCOS_REPO = "lucasnewman/vocos-mel-24khz"
@@ -94,12 +94,18 @@ def convert_vocos_upstream(w: Weights) -> Weights:
 
 
 def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits: Optional[int] = None,
-                    device: str | torch.device = "cuda", vocab_path: Optional[str] = None, vocoder=None):
+                    device: str | torch.device = "cuda", vocab_path: Optional[str] = None, vocoder=None,
+                    fp8: Optional[str] = None):
     """`vocoder`: None = resolve and REQUIRE one (reference behaviour), False = none (sample() returns mels),
-    or a callable mel -> waveform."""
+    or a callable mel -> waveform.  `fp8`: None = bf16, "tensor" or "block" = the DiT's FP8 mode with that weight /
+    activation scaling (DESIGN.md section 8); the weights (dequantised first for quantization_bits) are quantised to
+    e4m3 at pack time."""
     import os
     if quantization_bits is not None and quantization_bits not in (4, 8):
         raise ValueError(f"quantization_bits must be 4 or 8 (generate.py --q), got {quantization_bits}")
+    if fp8 is not None and fp8 not in FP8_SCALINGS:
+        raise ValueError(f"fp8 must be None or one of {FP8_SCALINGS}, got {fp8!r}")
+    fp8_kw = dict(fp8=fp8 is not None, fp8_scaling=fp8 or "tensor")
     if hf_model_name_or_path == "random":
         vp = vocab_path or os.environ.get("F5_VOCAB_PATH")
         if vp is not None:
@@ -108,7 +114,7 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
             vocab, vocab_source = ascii_vocab(), "ascii"
         cfg = BASE_CONFIG
         dit = DiT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, ff_mult=cfg.ff_mult, text_dim=cfg.text_dim,
-                  conv_layers=cfg.conv_layers, text_num_embeds=cfg.text_num_embeds, device=device)
+                  conv_layers=cfg.conv_layers, text_num_embeds=cfg.text_num_embeds, device=device, **fp8_kw)
         load_weights_distributed(dit, lambda: random_dit_weights(cfg, seed=1234))
         if vocoder is None:
             vocoder = Vocos(VocosConfig(), device).load_weights(random_vocos_weights()).decode
@@ -126,7 +132,7 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
     if quantization_bits is not None:                                            # cfm.py:450-453
         model_file, convert = f"model_v1_{quantization_bits}b.safetensors", False
     dit = DiT(dim=1024, depth=22, heads=16, ff_mult=2, text_dim=512, conv_layers=4,
-              text_num_embeds=len(vocab) - 1, text_mask_padding=True, device=device)     # cfm.py:459-469
+              text_num_embeds=len(vocab) - 1, text_mask_padding=True, device=device, **fp8_kw)     # cfm.py:459-469
 
     def weights_fn() -> Weights:
         w = load_file(str(path / model_file))

@@ -275,7 +275,8 @@ class DitBlockWeightsC(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in
                 ("qkv_w", "qkv_b", "out_w", "out_b", "ff1_w", "ff1_b", "ff2_w", "ff2_b", "qkv_w8", "ff1_w8", "out_w8",
                  "ff2_w8")] + \
-               [("qkv_s8", C.c_float), ("ff1_s8", C.c_float), ("out_s8", C.c_float), ("ff2_s8", C.c_float)]
+               [("qkv_s8", C.c_float), ("ff1_s8", C.c_float), ("out_s8", C.c_float), ("ff2_s8", C.c_float)] + \
+               [(n, C.c_void_p) for n in ("qkv_ws", "ff1_ws", "out_ws", "ff2_ws")]
 
 
 E4M3_MAX = 448.0
@@ -290,6 +291,34 @@ def quantize_e4m3(w: torch.Tensor):
         scale = 1.0
     q = (w / scale).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     return q.view(torch.uint8), scale
+
+
+FP8_SCALINGS = ("tensor", "block")
+
+
+def e4m3_block_scale(amax: torch.Tensor) -> torch.Tensor:
+    """The scale rule of the block-scaled FP8 mode, element-wise on fp32 amax >= 0: the smallest power of two s >= 2^-126
+    with amax <= 448 s, read off amax's exponent and mantissa bits exactly as the kernels do (ptx.cuh e4m3_block_scale);
+    1 for amax == 0; a non-finite amax is its own scale.  (The floor 2^-126 keeps 1 / s finite.)"""
+    a = amax.float().contiguous()
+    b = a.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    e, m = (b >> 23) & 0xFF, b & 0x7FFFFF
+    k = (e - 135 + (m > 0x600000).to(torch.int64)).clamp_min(-126)
+    s = ((k + 127) << 23).to(torch.int32).view(torch.float32)
+    s = torch.where(b == 0, torch.ones_like(s), s)
+    return torch.where(e == 0xFF, a, s)
+
+
+def quantize_e4m3_blocks(x: torch.Tensor, block: int = 64):
+    """Block-scaled e4m3 of an fp32 matrix [rows, cols]: one power-of-two scale per (row, `block` columns) (a whole row
+    with block = cols: the per-output-channel weight scale).  Returns (e4m3 codes as uint8 [rows, cols], scales fp32
+    [rows, cols / block]) with x ~= codes * scale, quantised as x * (1 / s) rounded to nearest even."""
+    x = x.detach().float()
+    r, c = x.shape
+    g = x.reshape(r, c // block, block)
+    s = e4m3_block_scale(g.abs().amax(dim=-1))
+    q = (g * (1.0 / s)[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    return q.view(torch.uint8).reshape(r, c), s
 
 
 class DitWeightsC(C.Structure):
@@ -348,10 +377,16 @@ class PackedDiT:
 
     ALIGN = 256
 
-    def __init__(self, cfg: DiTConfig, device: torch.device | str = "cuda", fp8: bool = False):
+    def __init__(self, cfg: DiTConfig, device: torch.device | str = "cuda", fp8: bool = False,
+                 fp8_scaling: str = "tensor"):
         self.cfg = cfg
         self.device = torch.device(device)
         self.fp8 = bool(fp8)           # also keep e4m3 copies of the QKV / FF1 weights (appended after the bf16 layout)
+        if fp8_scaling not in FP8_SCALINGS:
+            raise ValueError(f"fp8_scaling must be one of {FP8_SCALINGS}, not {fp8_scaling!r}")
+        # "tensor": one scale per weight tensor; "block": one power-of-two scale per output channel (the block-scaled mode)
+        self.fp8_scaling = fp8_scaling
+        self.fp8_block = self.fp8 and fp8_scaling == "block"
         self.ct_ld = _round_up(cfg.mel_dim + cfg.text_dim, 64)
         self.specs: Dict[str, _Spec] = {}
         off = 0
@@ -405,7 +440,12 @@ class PackedDiT:
             yield f"blk{i}.ff2_b", (D,), f32
         yield "proj_w", (c.mel_dim, D), bf
         yield "proj_b", (c.mel_dim,), f32
-        if self.fp8:       # FP8 mode: appended, so the bf16 prefix is the layout the C packer (f5_pack_weights) knows
+        if self.fp8_block:   # block-scaled FP8: per-channel e4m3 weights in the order a block reads them, + fp32 scales
+            for i in range(c.depth):
+                for n, (o, k) in (("qkv", (3 * D, D)), ("out", (D, D)), ("ff1", (F, D)), ("ff2", (D, F))):
+                    yield f"blk{i}.{n}_w8c", (o, k), torch.uint8
+                    yield f"blk{i}.{n}_s8c", (o,), f32
+        elif self.fp8:       # FP8 mode: appended, so the bf16 prefix is the layout the C packer (f5_pack_weights) knows
             for i in range(c.depth):
                 yield f"blk{i}.qkv_w8", (3 * D, D), torch.uint8
                 yield f"blk{i}.ff1_w8", (F, D), torch.uint8
@@ -476,7 +516,15 @@ class PackedDiT:
             self._put(f"blk{i}.ff1_b", g(p + "ff.ff.layers.0.layers.0.bias"))
             self._put(f"blk{i}.ff2_w", g(p + "ff.ff.layers.2.weight"))
             self._put(f"blk{i}.ff2_b", g(p + "ff.ff.layers.2.bias"))
-            if self.fp8:
+            if self.fp8_block:
+                for n, wt in (("qkv", torch.cat([g(p + f"attn.to_{n}.weight") for n in "qkv"], 0)),
+                              ("out", g(p + "attn.to_out.layers.0.weight")),
+                              ("ff1", g(p + "ff.ff.layers.0.layers.0.weight")),
+                              ("ff2", g(p + "ff.ff.layers.2.weight"))):
+                    q, sc = quantize_e4m3_blocks(wt, wt.shape[1])
+                    self.view(f"blk{i}.{n}_w8c").copy_(q)
+                    self._put(f"blk{i}.{n}_s8c", sc.reshape(-1))
+            elif self.fp8:
                 for j, (dst, wt) in enumerate(((f"blk{i}.qkv_w8", torch.cat([g(p + f"attn.to_{n}.weight") for n in "qkv"], 0)),
                                                (f"blk{i}.ff1_w8", g(p + "ff.ff.layers.0.layers.0.weight")),
                                                (f"blk{i}.out_w8", g(p + "attn.to_out.layers.0.weight")),
@@ -516,7 +564,12 @@ class PackedDiT:
         for i in range(c.depth):
             for n, _ in DitBlockWeightsC._fields_[:8]:
                 setattr(blks[i], n, ptr(f"blk{i}.{n}"))
-            if self.fp8:
+            if self.fp8_block:
+                for n in ("qkv", "ff1", "out", "ff2"):
+                    setattr(blks[i], f"{n}_w8", ptr(f"blk{i}.{n}_w8c"))
+                    setattr(blks[i], f"{n}_ws", ptr(f"blk{i}.{n}_s8c"))
+                    setattr(blks[i], f"{n}_s8", 1.0)
+            elif self.fp8:
                 sc = self.view("fp8_scales").cpu()
                 blks[i].qkv_w8, blks[i].ff1_w8 = ptr(f"blk{i}.qkv_w8"), ptr(f"blk{i}.ff1_w8")
                 blks[i].out_w8, blks[i].ff2_w8 = ptr(f"blk{i}.out_w8"), ptr(f"blk{i}.ff2_w8")

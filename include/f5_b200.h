@@ -132,6 +132,18 @@ typedef struct f5_gemm_args {
   int32_t out2_fp8;
   float acc_scale;
   int32_t out_fp8;        /* with out_bf16 = 1: `out` is written as e4m3 bytes instead (ldo in bytes, multiple of 16) */
+  /* Block-scaled FP8 (ABI 1.101; any of the four pointers non-NULL selects it).  Every scale is a power of two s, the
+   * smallest with amax <= 448 s (not below 2^-126; 1 for amax = 0), so that x ~= s * e4m3 is exact to scale.
+   * a_scale: fp32 [k/64][a_scale_ld] (a_scale_ld >= rows), the scale of `a` (ab_fp8) per (row, 64-column unit);
+   * w_scale: fp32 [n], the per-output-channel scale of `w` (the accumulator term is multiplied by acc_scale * w_scale);
+   * out_scale / out2_scale: fp32 [n/64][rows], written with the block-scaled e4m3 `out` (out_fp8) / `out2` (out2_fp8):
+   * each (row, 64-column unit) is quantised with its own scale (n % 64 == 0).  Built for the epilogues of the DiT's
+   * block-scaled mode only (RoPE QKV, residual fp32 + out2, GELU e4m3 out, Mish fp32 + out2). */
+  const float* a_scale;
+  int64_t a_scale_ld;
+  const float* w_scale;
+  float* out_scale;
+  float* out2_scale;
 } f5_gemm_args;
 
 int f5_gemm_bf16(const f5_gemm_args* args, void* stream);
@@ -153,6 +165,11 @@ int f5_attention_fwd(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out,
 int f5_attention_fwd_e4m3(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch,
                           int32_t frames, int32_t heads, int32_t head_dim, const int32_t* kv_len,
                           void* stream);
+/* block-scaled e4m3 output: each (row, head) of O is quantised with its own power-of-two scale (see f5_gemm_args.a_scale),
+ * written to scale_out fp32 [heads][batch*frames] — the a_scale of the block-scaled out-projection */
+int f5_attention_fwd_e4m3_scaled(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch,
+                                 int32_t frames, int32_t heads, int32_t head_dim, const int32_t* kv_len,
+                                 float* scale_out, void* stream);
 /* kept for ABI compatibility: accepts any `base` and returns 0; the attention kernel records no timeline */
 int f5_debug_attention_ts(void* base);
 
@@ -210,6 +227,10 @@ typedef struct f5_dit_block_weights {
    * out_w8 / ff2_w8 also the out-projection (attention writes e4m3) and FF2 (FF1 writes e4m3) run in FP8. */
   const void* qkv_w8; const void* ff1_w8; const void* out_w8; const void* ff2_w8;
   float qkv_s8, ff1_s8, out_s8, ff2_s8;
+  /* Block-scaled FP8 mode (ABI 1.101, optional): fp32 per-output-channel scales of the *_w8 weights (w[o] ~= s[o] *
+   * e4m3, *_s8 = 1).  With these and f5_dit_buffers.a_fp8 / a_fp8_scale / attn_scale / ff_scale all set, the four block
+   * GEMMs run on block-scaled e4m3 operands (see f5_gemm_args.a_scale). */
+  const float* qkv_ws; const float* ff1_ws; const float* out_ws; const float* ff2_ws;
 } f5_dit_block_weights;
 
 typedef struct f5_dit_weights {
@@ -279,6 +300,12 @@ typedef struct f5_dit_buffers {
   /* FP8 mode: e4m3 [rows, D] — the AdaLN-modulated operand of the QKV / FF1 GEMMs (written by the producing GEMM's
    * epilogue instead of a_bf16); requires the fused AdaLN buffers and blocks[i].qkv_w8 / ff1_w8.  NULL = bf16. */
   void* a_fp8;
+  /* Block-scaled FP8 mode (ABI 1.101): per (row, 64-column unit) scales, unit-major — fp32 [D/64][rows] of a_fp8, fp32
+   * [heads][rows] of the attention output (e4m3 in c_bf16), fp32 [ff_inner/64][rows] of the FF1 output (e4m3 in
+   * ff_bf16).  NULL = per-tensor FP8 (or bf16).  F5_FP8_LEVEL has no effect in this mode. */
+  float* a_fp8_scale;
+  float* attn_scale;
+  float* ff_scale;
 } f5_dit_buffers;
 
 /* step-invariant work, once per sample(): text embedding (dit.py:196-229), hoisted conditioning
