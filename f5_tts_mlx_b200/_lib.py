@@ -111,7 +111,23 @@ SYMBOLS: dict[str, tuple] = {
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_grn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                          C.c_int32, C.c_void_p]),
-    "f5_dit_precompute": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_ln_affine_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_ln_tab_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "f5_text_embed": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "f5_time_mlp": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_ode_update": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_void_p, C.c_float,
+                                C.c_void_p, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int64,
+                                C.c_int32, C.c_int32, C.c_void_p]),
+    "f5_cast_pad_bf16": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p]),
+    "f5_concat_cond_text": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "f5_duration_head": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p]),
+    "f5_grn_valid": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                               C.c_int32, C.c_void_p, C.c_void_p]),
+    "f5_dit_precompute":(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_dit_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "f5_dit_ln_tab_ld": (C.c_int64, [C.c_void_p]),
     "f5_ode_eval_times": (C.c_int, [C.POINTER(C.c_float), C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int32]),

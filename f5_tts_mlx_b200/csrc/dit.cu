@@ -92,7 +92,7 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
   // ---- TextEmbedding (dit.py:196-229) for the cond rows and, with CFG, the text-dropped rows ----
   if (int e = launch_text_embed_gather(b->text, B, b->text_len_max, N, C, w->text_emb, w->text_pos,
                                        w->text_max_pos, b->text_x, BU,
-                                       b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU), st))
+                                       b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU), st, 1, b->valid_len))
     return e;
   for (int l = 0; l < w->conv_layers; ++l) {
     const f5_convnext_weights& cw = w->text_blocks[l];

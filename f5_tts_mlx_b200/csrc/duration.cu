@@ -36,7 +36,7 @@ extern "C" int f5_duration_forward(const f5_duration_weights* w, const f5_durati
 
   // TextEmbedding with mask_padding=False: no row is zeroed, every ConvNeXt block sees all N rows
   if (int e = launch_text_embed_gather(b->text, B, b->text_len_max, N, C, w->text_emb, w->text_pos,
-                                       w->text_max_pos, b->text_x, B, B, st, /*mask_padding=*/0))
+                                       w->text_max_pos, b->text_x, B, B, st, /*mask_padding=*/0, /*valid_len=*/nullptr))
     return e;
   for (int l = 0; l < w->conv_layers; ++l) {
     const f5_convnext_weights& cw = w->text_blocks[l];

@@ -1,4 +1,6 @@
 // Host launchers + C-ABI entries for the HBM-bound kernels (elementwise.cuh).
+#include <string.h>
+
 #include "elementwise.cuh"
 #include "host_common.h"
 #include "launch.h"
@@ -86,12 +88,12 @@ int launch_grn(const void* h, void* y, float* nx_scratch, const float* gamma, co
 
 int launch_text_embed_gather(const int* text, int B, int nt, int N, int C, const float* emb,
                              const float* pos_table, int max_pos, float* x, int Bout,
-                             int drop_from, cudaStream_t st, int mask_padding) {
+                             int drop_from, cudaStream_t st, int mask_padding, const int* valid_len) {
   ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
   F5_REQUIRE(text && emb && pos_table && x, "text_embed_gather: null pointer");
   F5_REQUIRE(C % 4 == 0, "text_embed_gather: C %% 4");
   F5_CHECK_CUDA(launch_kernel(text_embed_gather_kernel, dim3(dim3(N, Bout)), dim3(128), 0, st, text, B, nt, N, C, emb, pos_table,
-                                                          max_pos, x, drop_from, mask_padding));
+                                                          max_pos, x, drop_from, mask_padding, valid_len));
   F5_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -146,6 +148,7 @@ int launch_duration_head(const float* x, int B, int N, int D, const int* len, co
     case 1024: F5_CHECK_CUDA(launch_kernel(duration_head_kernel<1024>, dim3(B), dim3(256), 0, st, x, N, len, norm_w, pred_w, out)); break;
     default: return set_error(F5_ERR_INVALID, "duration_head: unsupported dim %d", D);
   }
+  F5_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -174,6 +177,82 @@ int f5_grn(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gam
   if (int e = f5::device_check()) return e;
   return f5::launch_grn(h_bf16, y_bf16, nx_scratch, gamma, beta, batch, frames, channels,
                         (cudaStream_t)stream);
+}
+
+// ---- kernel test entries: each runs one launcher of the DiT / duration / Vocos paths alone ----
+
+int f5_ln_affine_f32(const float* x, float* y, int32_t rows, int32_t dim, const float* w, const float* b,
+                     void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_ln_f32(x, y, rows, dim, w, b, (cudaStream_t)stream);
+}
+
+int f5_ln_tab_prep(const float* mod, void* prep_bf16, int32_t times, int32_t depth, int32_t dim,
+                   int32_t mod_cols, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_ln_tab_prep(mod, prep_bf16, times, depth, dim, mod_cols, (cudaStream_t)stream);
+}
+
+int f5_text_embed(const int32_t* text, int32_t batch, int32_t text_cols, int32_t frames, int32_t channels,
+                  const float* emb, const float* pos_table, int32_t max_pos, float* x, int32_t batch_out,
+                  int32_t drop_from, int32_t mask_padding, const int32_t* valid_len, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_text_embed_gather(text, batch, text_cols, frames, channels, emb, pos_table, max_pos, x,
+                                      batch_out, drop_from, (cudaStream_t)stream, mask_padding, valid_len);
+}
+
+int f5_time_mlp(const float* tvals, int32_t times, int32_t dim, const float* w0, const float* b0,
+                const float* w2, const float* b2, float* t_emb, void* silu_bf16, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_time_mlp(tvals, times, dim, w0, b0, w2, b2, t_emb, silu_bf16, (cudaStream_t)stream);
+}
+
+int f5_ode_update(const float* v, int32_t ldv, int64_t null_row_offset, float cfg_strength,
+                  const float* y_base, float* y_out, float a, float* k_acc, float acc_w, int32_t acc_init,
+                  int32_t use_acc, void* y_bf16, int32_t ld_bf16, int64_t bf16_copy_row_offset, int32_t rows,
+                  int32_t d, void* stream) {
+  if (int e = f5::device_check()) return e;
+  F5_REQUIRE(v && rows > 0 && d > 0 && ldv >= d, "ode_update: bad arguments");
+  F5_REQUIRE(!y_out || y_base, "ode_update: y_out needs y_base");
+  F5_REQUIRE(!y_bf16 || ld_bf16 >= d, "ode_update: ld_bf16 < d");
+  f5::OdeUpdateParams p;
+  memset(&p, 0, sizeof(p));
+  p.v = v; p.ldv = ldv; p.null_row_offset = null_row_offset; p.cfg_strength = cfg_strength;
+  p.y_base = y_base; p.y_out = y_out; p.a = a;
+  p.k_acc = k_acc; p.acc_w = acc_w; p.acc_init = acc_init; p.use_acc = use_acc;
+  p.y_bf16 = reinterpret_cast<__nv_bfloat16*>(y_bf16); p.ld_bf16 = ld_bf16;
+  p.bf16_copy_row_offset = bf16_copy_row_offset;
+  p.rows = rows; p.d = d;
+  return f5::launch_ode_update(p, (cudaStream_t)stream);
+}
+
+int f5_cast_pad_bf16(const float* src, int32_t d, void* dst, int32_t ld, int32_t rows, int64_t copy_row_offset,
+                     void* stream) {
+  if (int e = f5::device_check()) return e;
+  F5_REQUIRE(src && dst && rows > 0 && ld >= d, "cast_pad_bf16: bad arguments");
+  return f5::launch_cast_pad_bf16(src, d, dst, ld, rows, copy_row_offset, (cudaStream_t)stream);
+}
+
+int f5_concat_cond_text(const float* cond, int32_t dc, int32_t batch_cond, int32_t frames, const float* text,
+                        int32_t dt, void* dst, int32_t ld, int32_t rows, int32_t drop_from_row,
+                        const int32_t* cond_len, void* stream) {
+  if (int e = f5::device_check()) return e;
+  F5_REQUIRE(cond && text && dst && rows > 0 && ld >= dc + dt, "concat_cond_text: bad arguments");
+  return f5::launch_concat_cond_text(cond, dc, batch_cond, frames, text, dt, dst, ld, rows, drop_from_row,
+                                     (cudaStream_t)stream, cond_len);
+}
+
+int f5_duration_head(const float* x, int32_t batch, int32_t frames, int32_t dim, const int32_t* len,
+                     const float* norm_w, const float* pred_w, float* out, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_duration_head(x, batch, frames, dim, len, norm_w, pred_w, out, (cudaStream_t)stream);
+}
+
+int f5_grn_valid(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gamma, const float* beta,
+                 int32_t batch, int32_t frames, int32_t channels, const int32_t* valid_len, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_grn(h_bf16, y_bf16, nx_scratch, gamma, beta, batch, frames, channels,
+                        (cudaStream_t)stream, valid_len);
 }
 
 }  // extern "C"

@@ -251,19 +251,23 @@ grn_apply_kernel(const __nv_bfloat16* __restrict__ h, __nv_bfloat16* __restrict_
 // computed BEFORE the CFG drop, drop -> id 0, Embedding gather, + sinusoid table row
 // min(n, 4095) (rope.py:76-84), masked rows -> 0.  text: int32 [B, nt] (pad -1).
 // Output x: fp32 [Bout, N, C].  Utterance bo reads text row (bo % B); rows bo >= drop_from are the
-// CFG "uncond" copies (ids dropped to 0, mask still from the real text).
+// CFG "uncond" copies (ids dropped to 0, mask still from the real text).  valid_len (frame bucketing,
+// may be NULL): rows n >= valid_len[bo] do not exist in the reference, whose text is truncated to the
+// real N — they are written as zeros, so the first dwconv7 sees zero padding there.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
 text_embed_gather_kernel(const int* __restrict__ text, int B, int nt, int N, int C,
                          const float* __restrict__ emb, const float* __restrict__ pos_table,
-                         int max_pos, float* __restrict__ x, int drop_from, int mask_padding) {
+                         int max_pos, float* __restrict__ x, int drop_from, int mask_padding,
+                         const int* __restrict__ valid_len) {
   pdl_launch_dependents();
   pdl_wait();
   const int n = blockIdx.x, bo = blockIdx.y;
   const int b = bo % B;
   int id = 0;
   if (n < nt) id = text[(size_t)b * nt + n] + 1;
-  const bool masked = mask_padding && (id == 0);   // DurationTransformer: mask_padding=False (duration.py:118-120)
+  const bool beyond = valid_len != nullptr && n >= valid_len[bo];
+  const bool masked = beyond || (mask_padding && (id == 0));   // DurationTransformer: mask_padding=False (duration.py:118-120)
   if (bo >= drop_from) id = 0;
   const int p = n < max_pos ? n : max_pos - 1;
   const float4* er = reinterpret_cast<const float4*>(emb + (size_t)id * C);

@@ -27,7 +27,8 @@ int launch_grn(const void* h, void* y, float* nx_scratch, const float* gamma, co
                int B, int N, int C, cudaStream_t st, const int* valid_len = nullptr);
 int launch_text_embed_gather(const int* text, int B, int nt, int N, int C, const float* emb,
                              const float* pos_table, int max_pos, float* x, int Bout,
-                             int drop_from, cudaStream_t st, int mask_padding = 1);
+                             int drop_from, cudaStream_t st, int mask_padding = 1,
+                             const int* valid_len = nullptr);
 int launch_time_mlp(const float* tvals, int T, int D, const float* w0, const float* b0,
                     const float* w2, const float* b2, float* t_emb, void* silu_bf16,
                     cudaStream_t st);

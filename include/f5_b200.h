@@ -194,6 +194,45 @@ int f5_grn(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gam
            const float* beta, int32_t batch, int32_t frames, int32_t channels, void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
+ * Kernel test entries: each runs one kernel that the model paths otherwise reach only inside
+ * f5_dit_precompute / f5_ode_sample / f5_duration_forward / f5_vocos_decode, with the same arguments.
+ * f5_ln_affine_f32    : affine LayerNorm with fp32 output (the Vocos backbone norm).
+ * f5_ln_tab_prep      : the fused-AdaLN operand rows hi/lo(1 + scale), hi/lo(shift) of every LN site.
+ *                       mod fp32 [times, mod_cols]; prep bf16 [2 depth + 1][4 times][dim].
+ * f5_text_embed       : TextEmbedding's gather (ids + 1, CFG drop from row drop_from, embedding +
+ *                       position table, masked rows 0).  x fp32 [batch_out, frames, channels];
+ *                       valid_len int32 [batch_out] or NULL: rows beyond it are written as zeros.
+ * f5_time_mlp         : TimestepEmbedding; t_emb fp32 [times, dim] (or NULL), silu_bf16 [times, dim].
+ * f5_ode_update       : CFG combine + explicit-solver stage update (see f5_ode_sample).
+ * f5_cast_pad_bf16    : fp32 [rows, d] -> bf16 [rows, ld], zero columns d..ld, optional row copy.
+ * f5_concat_cond_text : [cond | text | 0] as bf16 [rows, ld]; cond_len int32 [batch_cond] or NULL.
+ * f5_duration_head    : RMSNorm, masked mean over len[b] frames, Linear(dim -> 1), Softplus.
+ * f5_grn_valid        : f5_grn with valid_len int32 [batch] (frames beyond it excluded from the norm).
+ * ------------------------------------------------------------------------------------------ */
+int f5_ln_affine_f32(const float* x, float* y, int32_t rows, int32_t dim, const float* w, const float* b,
+                     void* stream);
+int f5_ln_tab_prep(const float* mod, void* prep_bf16, int32_t times, int32_t depth, int32_t dim,
+                   int32_t mod_cols, void* stream);
+int f5_text_embed(const int32_t* text, int32_t batch, int32_t text_cols, int32_t frames, int32_t channels,
+                  const float* emb, const float* pos_table, int32_t max_pos, float* x, int32_t batch_out,
+                  int32_t drop_from, int32_t mask_padding, const int32_t* valid_len, void* stream);
+int f5_time_mlp(const float* tvals, int32_t times, int32_t dim, const float* w0, const float* b0,
+                const float* w2, const float* b2, float* t_emb, void* silu_bf16, void* stream);
+int f5_ode_update(const float* v, int32_t ldv, int64_t null_row_offset, float cfg_strength,
+                  const float* y_base, float* y_out, float a, float* k_acc, float acc_w, int32_t acc_init,
+                  int32_t use_acc, void* y_bf16, int32_t ld_bf16, int64_t bf16_copy_row_offset, int32_t rows,
+                  int32_t d, void* stream);
+int f5_cast_pad_bf16(const float* src, int32_t d, void* dst, int32_t ld, int32_t rows, int64_t copy_row_offset,
+                     void* stream);
+int f5_concat_cond_text(const float* cond, int32_t dc, int32_t batch_cond, int32_t frames, const float* text,
+                        int32_t dt, void* dst, int32_t ld, int32_t rows, int32_t drop_from_row,
+                        const int32_t* cond_len, void* stream);
+int f5_duration_head(const float* x, int32_t batch, int32_t frames, int32_t dim, const int32_t* len,
+                     const float* norm_w, const float* pred_w, float* out, void* stream);
+int f5_grn_valid(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gamma, const float* beta,
+                 int32_t batch, int32_t frames, int32_t channels, const int32_t* valid_len, void* stream);
+
+/* ------------------------------------------------------------------------------------------ *
  * DiT (dit.py:331-401) and the ODE loop of F5TTS.sample (cfm.py:340-393).
  *
  * Weight layout ("packed"): what f5_tts_mlx_b200.weights.pack_dit() produces from the MLX

@@ -490,6 +490,33 @@ def test_frame_bucketing_one_plan_for_many_lengths_same_results(gate):
     assert len(plans) == 1 and bucketed.last_plan.session.frames == 256
 
 
+def test_frame_bucketing_text_longer_than_frames(gate):
+    """A bucketed session (frames = the 128-row bucket, the real N in valid_len) whose text has more real tokens than
+    N.  The reference truncates the text to N, so the bucket rows N.. must hold zeros when the first ConvNeXt block's
+    depthwise conv reads them as the right neighbours of rows N-3 .. N-1.  sample() cannot reach this case (it makes
+    the duration at least the text length + 1), but a session driven directly can."""
+    import torch.nn.functional as F
+    cfg, W, model = gate
+    g = torch.Generator().manual_seed(33)
+    for N, nt in ((150, 200), (201, 260)):
+        NB, tcols = -(-N // 128) * 128, -(-nt // 32) * 32
+        text = F.pad(torch.randint(0, 2545, (1, nt), generator=g, dtype=torch.int32), (0, tcols - nt), value=-1)
+        x = torch.randn(1, N, 100, generator=g)
+        cond = torch.randn(1, N, 100, generator=g) * 2 - 1
+        t = torch.tensor(0.37)
+        exact = model(x.to(dev), cond.to(dev), text.to(dev), t).cpu()
+        s = model.session(1, NB, 1, False, tcols, False, bucketed=True)
+        s.set_inputs(text, F.pad(cond, (0, 0, 0, NB - N)).to(dev), t.reshape(1).to(dev), None, frames_valid=N)
+        s.c.drop_flags = 0
+        s.y_bf16.zero_()
+        s.y_bf16[:N, :100].copy_(x[0])
+        model.precompute(s)
+        got = model.forward_session(s, 0).view(1, NB, 100)[:, :N].cpu()
+        assert rel(got, exact) < 1e-3, (N, nt, rel(got, exact))
+        ref = O.dit_forward(x, cond, text, t, False, False, None, W, ocfg_of(cfg))
+        assert rel(got, ref) < 1e-2
+
+
 def test_fp8_mode_forward_within_derived_drift(base):
     """DiT(fp8=True): the four GEMMs of every block on e4m3 operands (weights quantised per tensor at pack time,
     activations written as e4m3 by the producing kernels) — the H100 analogue of the reference's lossy `--q`
