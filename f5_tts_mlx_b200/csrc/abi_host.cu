@@ -89,8 +89,8 @@ Layout make_layout(const f5_dit_dims* d) {
 
 int check_dims(const f5_dit_dims* d) {
   F5_REQUIRE(d != nullptr, "null f5_dit_dims");
-  F5_REQUIRE(d->dim % 128 == 0 && d->dim >= 256 && d->dim <= 1024 && d->dim == d->heads * 64, "f5_dit_dims: dim %d / heads %d", d->dim,
-             d->heads);
+  F5_REQUIRE(d->dim % 128 == 0 && d->dim >= 256 && d->dim <= 1024 && 64 % (d->dim / 16) == 0 && d->dim == d->heads * 64,
+             "f5_dit_dims: dim %d / heads %d", d->dim, d->heads);
   F5_REQUIRE(d->depth > 0 && d->ff_inner > 0 && d->mel_dim > 0 && d->mel_dim <= 128 && d->text_dim % 64 == 0 && d->conv_layers >= 0 &&
                  d->text_num_embeds > 0,
              "f5_dit_dims: bad field");

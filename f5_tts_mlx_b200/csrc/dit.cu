@@ -37,8 +37,11 @@ static f5_gemm_args gemm_base(const void* a, int64_t lda, const void* w, int64_t
 
 static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b) {
   F5_REQUIRE(w && b, "dit: null weights/buffers");
-  F5_REQUIRE(w->dim % 128 == 0 && w->dim >= 256 && w->dim <= 1024,
-             "dit: dim %d unsupported (128 | dim, 256..1024: the grouped conv packs 16 groups of <= 64 channels)", w->dim);
+  // the implicit grouped conv reads 64-channel blocks, so each of its 16 groups (dim/16 channels) must lie inside one
+  // block: dim/16 divides 64, which within 256..1024 leaves 256, 512 and 1024
+  F5_REQUIRE(w->dim % 128 == 0 && w->dim >= 256 && w->dim <= 1024 && 64 % (w->dim / 16) == 0,
+             "dit: dim %d unsupported (256, 512 or 1024: the conv's dim/16-channel groups must tile 64-channel blocks)",
+             w->dim);
   F5_REQUIRE(w->dim == w->heads * 64, "dit: dim %d != heads %d * 64", w->dim, w->heads);
   F5_REQUIRE(w->mel_dim % 4 == 0 && w->mel_dim <= 128, "dit: mel_dim %d", w->mel_dim);
   F5_REQUIRE(w->blocks && w->depth > 0, "dit: no blocks");

@@ -28,7 +28,9 @@ extern "C" int f5_duration_forward(const f5_duration_weights* w, const f5_durati
                                    void* stream_) {
   if (int e = device_check()) return e;
   F5_REQUIRE(w && b, "f5_duration_forward: null pointer");
-  F5_REQUIRE(w->dim % 128 == 0 && w->dim == w->heads * 64, "f5_duration_forward: dim %d heads %d", w->dim, w->heads);
+  // the grouped conv's dim/16-channel groups must tile its 64-channel blocks (check_common in dit.cu)
+  F5_REQUIRE(w->dim % 128 == 0 && 64 % (w->dim / 16) == 0 && w->dim == w->heads * 64,
+             "f5_duration_forward: dim %d heads %d", w->dim, w->heads);
   F5_REQUIRE(b->batch > 0 && b->frames > 0, "f5_duration_forward: bad shape");
   cudaStream_t st = (cudaStream_t)stream_;
   const int D = w->dim, N = b->frames, B = b->batch, R = B * N, F = w->ff_inner;

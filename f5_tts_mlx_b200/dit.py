@@ -155,8 +155,10 @@ class DiT:
             text_dim = mel_dim
         if dim_head != 64 or dim != heads * dim_head:
             raise ValueError("libf5b200 supports dim_head == 64 and dim == heads * 64")
-        if dim % 128 != 0 or not (256 <= dim <= 1024):
-            raise ValueError("libf5b200 supports 256 <= dim <= 1024, dim a multiple of 128 (see check_common in csrc/dit.cu)")
+        if dim not in (256, 512, 1024):
+            # the implicit grouped conv reads 64-channel blocks: its dim/16-channel groups must tile them (64 % (dim/16) == 0)
+            raise ValueError(f"libf5b200 supports dim 256, 512 or 1024, not {dim}: the conv position embedding's dim/16-channel "
+                             "groups must tile 64-channel blocks (see check_common in csrc/dit.cu)")
         if not text_mask_padding:
             raise NotImplementedError("text_mask_padding=False is not on the accelerated path")
         if dropout != 0.0:

@@ -54,6 +54,9 @@ class DurationTransformer:
             text_dim = mel_dim
         if dim_head != 64 or dim != heads * dim_head:
             raise ValueError("libf5b200 supports dim_head == 64 and dim == heads * 64")
+        if dim % 128 != 0 or 64 % (dim // 16) != 0:
+            raise ValueError(f"libf5b200 supports dim 128, 256, 512 or 1024, not {dim}: the conv position embedding's "
+                             "dim/16-channel groups must tile 64-channel blocks")
         if conv_layers <= 0:
             raise NotImplementedError("conv_layers == 0 (no positional table) is not on the accelerated path")
         self.dim, self.depth, self.heads, self.ff_mult = dim, depth, heads, ff_mult

@@ -68,7 +68,18 @@ def test_rope_table_matches_oracle_freqs():
     assert torch.equal(text_pos_table(512), O.precompute_freqs_cis(512, 4096))
 
 
-@pytest.mark.parametrize("dim", [1024, 512])
+@pytest.mark.parametrize("dim", [384, 640, 768, 896])
+def test_dim_whose_conv_groups_straddle_64_channel_blocks_is_rejected_at_construction(dim):
+    """The implicit grouped conv reads 64-channel blocks, so its dim/16-channel groups must tile them.  Widths where
+    they straddle a block (dim/16 = 24, 40, 48, 56) are refused when the model is built, not at load time."""
+    from f5_tts_mlx_b200.duration import DurationTransformer
+    with pytest.raises(ValueError, match="64-channel blocks"):
+        DiT(dim=dim, heads=dim // 64, device="cpu")
+    with pytest.raises(ValueError, match="64-channel blocks"):
+        DurationTransformer(dim=dim, heads=dim // 64, conv_layers=2)
+
+
+@pytest.mark.parametrize("dim", [1024, 512, 256])
 def test_pack_grouped_conv_is_the_grouped_conv(dim):
     """The implicit-GEMM weight layout ([O, 31*64] tap-major, block-diagonal by 64 channels) computes
     exactly Conv1d(groups=16): emulate the kernel's access pattern on the CPU."""
