@@ -55,14 +55,13 @@ class GemmArgs(C.Structure):
         ("bias", C.c_void_p),
         ("out", C.c_void_p), ("ldo", C.c_int64),
         ("resid", C.c_void_p), ("ldr", C.c_int64),
-        ("gate", C.c_void_p), ("gate_ld", C.c_int64),
+        ("gate", C.c_void_p),
         ("row_len", C.c_void_p),
         ("rope", C.c_void_p), ("rope_cols", C.c_int32),
         ("q_scale", C.c_float), ("q_cols", C.c_int32),
         ("tile_n", C.c_int32),
         ("out2_bf16", C.c_void_p), ("ldo2", C.c_int64),
-        ("variant", C.c_int32), ("w_static", C.c_int32),
-        ("debug_ts", C.c_void_p),
+        ("w_static", C.c_int32),
         ("prefetch", C.c_void_p), ("prefetch_bytes", C.c_int64),
         ("ln_scale", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_in_stats", C.c_void_p),
         ("ln_tab", C.c_void_p), ("ln_tab_ld", C.c_int64),
@@ -92,13 +91,9 @@ SYMBOLS: dict[str, tuple] = {
     "f5_device_check": (C.c_int, []),
     "f5_struct_sizes": (C.c_int, [C.POINTER(C.c_int32), C.c_int32]),
     "f5_launch_count": (C.c_longlong, []),
-    "f5_prof_enable": (C.c_int, [C.c_int]),
-    "f5_prof_summary": (C.c_int, [C.POINTER(C.c_double), C.c_int]),
     "f5_prof_graph_begin": (C.c_int, [C.c_void_p, C.c_int32]),
     "f5_prof_graph_meta": (C.c_int, [C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int32]),
     "f5_gemm_bf16": (C.c_int, [C.POINTER(GemmArgs), C.c_void_p]),
-    "f5_debug_gemm_ts": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32]),
-    "f5_debug_attention_ts": (C.c_int, [C.c_void_p]),
     "f5_attention_fwd": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "f5_attention_fwd_e4m3": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32,

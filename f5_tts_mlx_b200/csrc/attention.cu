@@ -2,12 +2,6 @@
 #include "attention_sm90.cuh"
 #include "host_common.h"
 
-// The attention kernel records no per-tile timeline; the entry point stays for ABI compatibility.
-extern "C" int f5_debug_attention_ts(void* base) {
-  (void)base;
-  return 0;
-}
-
 static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch, int32_t frames,
                           int32_t heads, int32_t head_dim, const int32_t* kv_len, int out_fp8, void* stream_,
                           float* scale_out = nullptr);
@@ -55,7 +49,7 @@ static int attention_impl(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
   p.scale_out = scale_out;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfScope ps(PROF_ATTN, 4.0 * batch * heads * (double)frames * frames * 64.0,
-               2.0 * batch * (double)frames * heads * 64.0 * 4.0, stream);
+               2.0 * batch * (double)frames * heads * 64.0 * 4.0);
   p.prof = ps.slot;
   auto launch = [&](auto kern, SmemAttrOnce& once, dim3 grid, int threads, int smem) -> int {
     F5_CHECK_CUDA(ensure_dyn_smem(once, kern, smem));

@@ -53,7 +53,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p)
   const int b = blockIdx.z;
   const int HD = p.H * 64;
 
-  if (warp == 0 && F5_ELECT_LANE()) {
+  if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tma_qkv);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
@@ -74,7 +74,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tma_qkv, const AttnParams p)
 
   if (warp < 4) {
     // ===================== TMA producer =====================
-    if (warp == 0 && F5_ELECT_LANE()) {
+    if (warp == 0 && elect_one()) {
       mbar_expect_tx(q_full, 16384);
       tma_load_3d(smem + AttnSmem::kQ, &tma_qkv, q_full, h * 64, q0, b);
       for (int j = 0; j < num_kv; ++j) {

@@ -154,8 +154,7 @@ int f5_mel_forward(const float* audio, int32_t batch, int32_t samples, const flo
   F5_REQUIRE(batch > 0 && samples > 0 && frames > 0 && n_mels > 0, "f5_mel_forward: bad shape");
   F5_REQUIRE(frames <= samples / hop, "f5_mel_forward: frames %d > samples/hop %d", frames,
              samples / hop);
-  ProfScope ps(PROF_OTHER, 0.0, 4.0 * batch * (double)samples + 4.0 * batch * (double)frames * n_mels,
-               (cudaStream_t)stream);
+  ProfScope ps(PROF_OTHER, 0.0, 4.0 * batch * (double)samples + 4.0 * batch * (double)frames * n_mels);
   F5_CHECK_CUDA(launch_kernel(mel_kernel, dim3(dim3(cdiv(frames, kMelWarps), batch)), dim3(kMelWarps * 32), 0, (cudaStream_t)stream, 
       audio, samples, window, filters, n_mels, hop, out, frames));
   F5_CHECK_CUDA(cudaGetLastError());
@@ -170,7 +169,7 @@ int f5_istft(const float* h, int64_t ldh, int32_t batch, int32_t frames, const f
   F5_REQUIRE(ldh >= 1026, "f5_istft: ldh %lld < 1026", (long long)ldh);
   const int rows = batch * frames;
   cudaStream_t st = (cudaStream_t)stream;
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_CHECK_CUDA(launch_kernel(istft_frames_kernel, dim3(cdiv(rows, kMelWarps)), dim3(kMelWarps * 32), 0, st, h, (int)ldh, window,
                                                                        frames_scratch, rows));
   F5_CHECK_CUDA(launch_kernel(istft_ola_kernel, dim3(dim3(cdiv(out_len, 256), batch)), dim3(256), 0, st, frames_scratch, window, frames,
@@ -218,7 +217,7 @@ int f5_vocos_decode(const f5_vocos_weights* w, const f5_vocos_buffers* b, const 
       g.a = b->i_bf16; g.lda = Ci; g.w = bw.pw2_w; g.ldw = Ci; g.m = R; g.n = D; g.k = Ci;
       g.num_batches = 1; g.conv_taps = 1;
       g.bias = bw.pw2_b; g.out = b->x; g.ldo = D; g.q_scale = 1.f;
-      g.gate = bw.gamma; g.gate_ld = 0;           // layer scale: per-channel gamma
+      g.gate = bw.gamma;                          // layer scale: per-channel gamma
       g.resid = b->x; g.ldr = D;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }

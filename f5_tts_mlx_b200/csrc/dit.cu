@@ -6,8 +6,9 @@
 //   * cond·Wc + text·Wt + b of InputEmbedding.proj    -> once per sample (dit.py:249)
 //   * TimestepEmbedding + all 23 AdaLN linears         -> one GEMM over all time points (dit.py:389,267,286)
 // and the two unbatched CFG passes (cfm.py:342-363) run as one forward over a doubled batch.
-#include <stdlib.h>
 #include <string.h>
+
+#include <initializer_list>
 
 #include "host_common.h"
 #include "launch.h"
@@ -35,7 +36,60 @@ static f5_gemm_args gemm_base(const void* a, int64_t lda, const void* w, int64_t
   return g;
 }
 
-static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b) {
+// What f5_dit_forward runs, chosen by the buffers the caller binds (see f5_dit_buffers in include/f5_b200.h)
+struct DitMode {
+  bool fused;   // AdaLN LayerNorm folded into the GEMM epilogues (ln_stats / ln_tab / ln_prep)
+  bool fp8;     // the four block GEMMs on e4m3 operands (a_fp8)
+  bool blk8;    // ... with block scales (a_fp8_scale / attn_scale / ff_scale)
+};
+
+struct NamedPtr { const char* name; const void* p; };
+// 0 when every pointer of `ptrs` is set, else F5_ERR_INVALID naming the NULL ones (of blocks[block] when block >= 0)
+static int need_all(const char* mode, int block, std::initializer_list<NamedPtr> ptrs) {
+  char missing[128] = "";
+  for (const NamedPtr& n : ptrs) {
+    const size_t len = strlen(missing);
+    if (n.p == nullptr) snprintf(missing + len, sizeof(missing) - len, "%s%s", len ? ", " : "", n.name);
+  }
+  if (missing[0] == 0) return 0;
+  if (block < 0) return set_error(F5_ERR_INVALID, "dit: %s needs %s", mode, missing);
+  return set_error(F5_ERR_INVALID, "dit: %s needs %s of blocks[%d]", mode, missing, block);
+}
+
+// A partly bound mode is an error rather than a quiet fall-back to another mode.
+static int check_mode(const f5_dit_weights* w, const f5_dit_buffers* b, DitMode& m) {
+  m.fused = b->ln_stats || b->ln_tab || b->ln_prep;
+  m.blk8 = b->a_fp8_scale || b->attn_scale || b->ff_scale;
+  m.fp8 = b->a_fp8 || m.blk8;
+  if (m.fused)
+    if (int e = need_all("fused AdaLN", -1, {{"ln_stats", b->ln_stats}, {"ln_tab", b->ln_tab}, {"ln_prep", b->ln_prep}}))
+      return e;
+  if (m.fp8) {
+    F5_REQUIRE(m.fused, "dit: FP8 needs the fused AdaLN buffers ln_stats, ln_tab and ln_prep");
+    if (int e = need_all("FP8", -1, {{"a_fp8", b->a_fp8}})) return e;
+  }
+  if (m.blk8)
+    if (int e = need_all("block-scaled FP8", -1, {{"a_fp8_scale", b->a_fp8_scale}, {"attn_scale", b->attn_scale},
+                                                  {"ff_scale", b->ff_scale}}))
+      return e;
+  for (int l = 0; m.fp8 && l < w->depth; ++l) {
+    const f5_dit_block_weights& bw = w->blocks[l];
+    if (int e = need_all("FP8", l, {{"qkv_w8", bw.qkv_w8}, {"ff1_w8", bw.ff1_w8}, {"out_w8", bw.out_w8},
+                                    {"ff2_w8", bw.ff2_w8}}))
+      return e;
+    // per-channel scales without the block-scale buffers would run the per-tensor mode on per-channel weights
+    F5_REQUIRE(m.blk8 || !(bw.qkv_ws || bw.ff1_ws || bw.out_ws || bw.ff2_ws),
+               "dit: blocks[%d] has per-channel weight scales (*_ws): block-scaled FP8 needs a_fp8_scale, attn_scale "
+               "and ff_scale", l);
+    if (m.blk8)
+      if (int e = need_all("block-scaled FP8", l, {{"qkv_ws", bw.qkv_ws}, {"ff1_ws", bw.ff1_ws}, {"out_ws", bw.out_ws},
+                                                   {"ff2_ws", bw.ff2_ws}}))
+        return e;
+  }
+  return 0;
+}
+
+static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b, DitMode& mode) {
   F5_REQUIRE(w && b, "dit: null weights/buffers");
   // the implicit grouped conv reads 64-channel blocks, so each of its 16 groups (dim/16 channels) must lie inside one
   // block: dim/16 divides 64, which within 256..1024 leaves 256, 512 and 1024
@@ -46,35 +100,11 @@ static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b) {
   F5_REQUIRE(w->mel_dim % 4 == 0 && w->mel_dim <= 128, "dit: mel_dim %d", w->mel_dim);
   F5_REQUIRE(w->blocks && w->depth > 0, "dit: no blocks");
   F5_REQUIRE(b->batch > 0 && b->frames > 0 && b->n_times > 0, "dit: bad buffer shape");
-  return 0;
-}
-
-// Tuning aid: F5_TUNE="qkv=2:192,out=1:128,ff1=1:128,ff2=1:64" overrides (variant:tile_n) of the block's GEMMs so the
-// kernel-variant space can be measured in situ (bench.py) without rebuilding; unset = the launcher's own heuristics.
-struct GemmTune { int variant, tile_n; };
-static GemmTune tune_of(const char* key) {
-  GemmTune t = {0, 0};
-  const char* env = getenv("F5_TUNE");
-  if (!env) return t;
-  const char* p = strstr(env, key);
-  if (!p) return t;
-  p += strlen(key);
-  if (*p != '=') return t;
-  t.variant = atoi(p + 1);
-  const char* c = strchr(p, ':');
-  const char* comma = strchr(p, ',');
-  if (c && (!comma || c < comma)) t.tile_n = atoi(c + 1);
-  return t;
+  return check_mode(w, b, mode);
 }
 
 static long long ln_tab_ld(const f5_dit_weights* w) {
   return (long long)w->depth * (3 * w->dim + w->ff_inner) + 128;
-}
-// F5_LN_FUSED=0 keeps the separate LayerNorm+modulate launches even when the fused-AdaLN buffers are present
-static bool ln_fused(const f5_dit_buffers* b) {
-  static int env = -1;
-  if (env < 0) { const char* v = getenv("F5_LN_FUSED"); env = (v && v[0] == '0') ? 0 : 1; }
-  return env && b->ln_stats && b->ln_tab && b->ln_prep;
 }
 
 }  // namespace f5
@@ -85,7 +115,8 @@ extern "C" int64_t f5_dit_ln_tab_ld(const f5_dit_weights* w) { return w ? ln_tab
 
 extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* b, void* stream_) {
   if (int e = device_check()) return e;
-  if (int e = check_common(w, b)) return e;
+  DitMode mode;
+  if (int e = check_common(w, b, mode)) return e;
   cudaStream_t st = (cudaStream_t)stream_;
   const int D = w->dim, N = b->frames, B = b->batch;
   const int BU = (b->cfg ? 2 : 1) * B;  // row-utterances
@@ -139,7 +170,7 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
   // ---- fused AdaLN: c1 = (1 + scale) W^T and c2 = shift W^T of every consuming Linear, for all times ----
-  if (ln_fused(b)) {
+  if (mode.fused) {
     const int NM = w->depth * 6 * D + 2 * D, T = b->n_times, F = w->ff_inner;
     const long long ld = ln_tab_ld(w);
     if (int e = launch_ln_tab_prep(b->mod_table, b->ln_prep, T, w->depth, D, NM, st)) return e;
@@ -160,7 +191,8 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
 extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, int32_t ti,
                               void* stream_) {
   if (int e = device_check()) return e;
-  if (int e = check_common(w, b)) return e;
+  DitMode mode;
+  if (int e = check_common(w, b, mode)) return e;
   F5_REQUIRE(ti >= 0 && ti < b->n_times, "dit_forward: time_index %d out of [0,%d)", ti, b->n_times);
   cudaStream_t st = (cudaStream_t)stream_;
   const int D = w->dim, N = b->frames, F = w->ff_inner;
@@ -170,23 +202,12 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
   const float* mod = b->mod_table + (size_t)ti * NM;
   // weight prefetch chain: worthwhile while a GEMM's weights are comparable to its activations
   // (small batch); at large batch the activations evict them anyway and HBM is busy
-  static int pf_env = -1;
-  if (pf_env < 0) { const char* v = getenv("F5_PREFETCH"); pf_env = (v && v[0] == '0') ? 0 : 1; }
-  const bool prefetch = pf_env && R <= 16384;
-  const bool fused = ln_fused(b);
-  // FP8 mode of the QKV / FF1 GEMMs: e4m3 operand written by the producing epilogue, e4m3 weights (per-tensor scale)
-  const bool fp8 = fused && b->a_fp8 != nullptr && w->blocks[0].qkv_w8 != nullptr && w->blocks[0].ff1_w8 != nullptr;
-  // ... and of the out-projection / FF2 (A = attention output / GELU output, written as e4m3 by their producers into the
-  // first half of the bf16 buffers); F5_FP8_LEVEL=1 keeps those two in bf16 (A/B measurements)
-  static int fp8_level = -1;
-  if (fp8_level < 0) { const char* v = getenv("F5_FP8_LEVEL"); fp8_level = (v && v[0] == '1') ? 1 : 2; }
-  const bool fp8b = fp8 && fp8_level >= 2 && w->blocks[0].out_w8 != nullptr && w->blocks[0].ff2_w8 != nullptr;
-  // block-scaled FP8 (DESIGN.md section 8): per-channel weight scales and per-(row, 64-column unit) activation scales;
-  // all four block GEMMs run on e4m3 operands, whatever F5_FP8_LEVEL says
-  const f5_dit_block_weights& b0 = w->blocks[0];
-  const bool blk8 = fp8 && b0.out_w8 && b0.ff2_w8 && b0.qkv_ws && b0.ff1_ws && b0.out_ws && b0.ff2_ws &&
-                    b->a_fp8_scale && b->attn_scale && b->ff_scale;
-  static const GemmTune t_qkv = tune_of("qkv"), t_out = tune_of("out"), t_ff1 = tune_of("ff1"), t_ff2 = tune_of("ff2");
+  const bool prefetch = R <= 16384;
+  // FP8 mode: all four block GEMMs on e4m3 weights; the QKV / FF1 operand is written as e4m3 by the producing
+  // epilogue, the out-projection / FF2 operand (attention output / GELU output) by its producer into the first half of
+  // the bf16 buffer.  Block-scaled FP8 (DESIGN.md section 8) adds per-channel weight scales and per-(row, 64-column
+  // unit) activation scales.
+  const bool fused = mode.fused, fp8 = mode.fp8, blk8 = mode.blk8;
   const long long tab_ld = ln_tab_ld(w);
   const float* tab = fused ? b->ln_tab + (size_t)4 * ti * tab_ld : nullptr;   // this time's 4 operand rows
 
@@ -233,7 +254,6 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)l * (3 * D + F); g.ln_tab_ld = tab_ld; }
       if (fp8) { g.a = b->a_fp8; g.w = bw.qkv_w8; g.ab_fp8 = 1; g.acc_scale = bw.qkv_s8; }
       if (blk8) { g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.qkv_ws; g.acc_scale = 1.f; }
-      g.variant = t_qkv.variant; g.tile_n = t_qkv.tile_n;
       g.rows_per_batch = N; g.num_batches = BU;
       g.rope = b->rope; g.rope_cols = 2 * D; g.q_scale = 0.125f; g.q_cols = D;
       // weight prefetch chain (L2): while QKV runs, pull in out_w and ff1_w (contiguous in the pack)
@@ -245,7 +265,7 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       if (int e = f5_attention_fwd_e4m3_scaled(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
                                                b->seq_len ? b->seq_len : b->valid_len, b->attn_scale, st))
         return e;
-    } else if (int e = (fp8b ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads,
+    } else if (int e = (fp8 ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads,
                                                                          64, b->seq_len ? b->seq_len : b->valid_len, st)) {
       return e;
     }
@@ -253,20 +273,19 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       f5_gemm_args g = gemm_base(b->c_bf16, D, bw.out_w, D, R, D, D, b->x, D, false);
       g.bias = bw.out_b;
       g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->seq_len;
-      g.gate = m + 2 * D; g.gate_ld = 0;
+      g.gate = m + 2 * D;
       g.resid = b->x; g.ldr = D;
       if (prefetch) { g.prefetch = bw.ff1_w; g.prefetch_bytes = (int64_t)2 * F * D; }
       if (fused) {   // ff_norm
         g.ln_scale = m + 4 * D; g.ln_stats = b->ln_stats;
         g.out2_bf16 = fp8 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = fp8 ? 1 : 0;
       }
-      if (fp8b) { g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = bw.out_s8; }     // A = c_bf16's bytes, e4m3 [R, D]
+      if (fp8) { g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = bw.out_s8; }     // A = c_bf16's bytes, e4m3 [R, D]
       if (blk8) {
         g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.out_ws;
         g.a_scale = b->attn_scale; g.a_scale_ld = R; g.out2_scale = b->a_fp8_scale;
         if (prefetch) { g.prefetch = bw.ff1_w8; g.prefetch_bytes = (int64_t)F * D; }
       }
-      g.variant = t_out.variant; g.tile_n = t_out.tile_n;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
     if (!fused)
@@ -275,9 +294,9 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       f5_gemm_args g = gemm_base(b->a_bf16, D, bw.ff1_w, D, R, F, D, b->ff_bf16, F, true);
       g.bias = bw.ff1_b; g.act = F5_ACT_GELU_TANH;
       if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)l * (3 * D + F) + 3 * D; g.ln_tab_ld = tab_ld; }
-      if (fp8) { g.a = b->a_fp8; g.w = bw.ff1_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff1_s8; }
-      if (fp8b) g.out_fp8 = 1;                                                   // ff_bf16's bytes as e4m3 [R, F]
-      g.variant = t_ff1.variant; g.tile_n = t_ff1.tile_n;
+      if (fp8) {   // out: ff_bf16's bytes as e4m3 [R, F]
+        g.a = b->a_fp8; g.w = bw.ff1_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff1_s8; g.out_fp8 = 1;
+      }
       if (prefetch) { g.prefetch = bw.ff2_w; g.prefetch_bytes = (int64_t)2 * D * F; }
       if (blk8) {
         g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.ff1_ws; g.acc_scale = 1.f;
@@ -290,7 +309,7 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       f5_gemm_args g = gemm_base(b->ff_bf16, F, bw.ff2_w, F, R, D, F, b->x, D, false);
       g.bias = bw.ff2_b;
       g.rows_per_batch = N; g.num_batches = BU;
-      g.gate = m + 5 * D; g.gate_ld = 0;
+      g.gate = m + 5 * D;
       g.resid = b->x; g.ldr = D;
       if (prefetch && l + 1 < w->depth) {
         g.prefetch = w->blocks[l + 1].qkv_w; g.prefetch_bytes = (int64_t)2 * 3 * D * D;
@@ -300,7 +319,7 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
         g.ln_stats = b->ln_stats; g.out2_bf16 = b->a_bf16; g.ldo2 = D;
         if (fp8 && l + 1 < w->depth) { g.out2_bf16 = b->a_fp8; g.out2_fp8 = 1; }   // proj_out (after the last block) stays bf16
       }
-      if (fp8b) { g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff2_s8; }
+      if (fp8) { g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff2_s8; }
       if (blk8) {
         g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.ff2_ws;
         g.a_scale = b->ff_scale; g.a_scale_ld = R;
@@ -308,7 +327,6 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
         g.prefetch = nullptr; g.prefetch_bytes = 0;
         if (prefetch && l + 1 < w->depth) { g.prefetch = w->blocks[l + 1].qkv_w8; g.prefetch_bytes = (int64_t)3 * D * D; }
       }
-      g.variant = t_ff2.variant; g.tile_n = t_ff2.tile_n;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
   }
@@ -356,7 +374,8 @@ extern "C" int f5_ode_sample(const f5_dit_weights* w, const f5_dit_buffers* b, c
                              int32_t steps, int32_t method, float cfg_strength, float* y,
                              float* trajectory, float* scratch, void* stream_) {
   if (int e = device_check()) return e;
-  if (int e = check_common(w, b)) return e;
+  DitMode mode;
+  if (int e = check_common(w, b, mode)) return e;
   F5_REQUIRE(t && steps >= 2 && y, "ode_sample: bad arguments");
   F5_REQUIRE(method >= 0 && method <= 2, "ode_sample: unknown method %d", method);
   F5_REQUIRE((cfg_strength >= 1e-5f) == (b->cfg != 0),

@@ -14,7 +14,7 @@ static int launch_ln_any(const float* x, void* yo, int rows, int dim, int rows_p
   F5_REQUIRE(x && yo && scale && shift, "ln_modulate: null pointer");
   F5_REQUIRE(rows > 0, "ln_modulate: rows=%d", rows);
   const int blocks = cdiv(rows * 32, 256);
-  ProfScope ps(PROF_LN, 0.0, (double)rows * dim * (OUT_F32 ? 8.0 : 6.0), st);
+  ProfScope ps(PROF_LN, 0.0, (double)rows * dim * (OUT_F32 ? 8.0 : 6.0));
   switch (dim) {
 #define F5_LN_CASE(DD)                                                                         \
   case DD:                                                                                     \
@@ -44,7 +44,7 @@ int launch_ln_f32(const float* x, float* y, int rows, int dim, const float* w, c
 }
 
 int launch_ln_tab_prep(const float* mod, void* prep_bf16, int T, int L, int D, int NM, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(mod && prep_bf16 && T > 0 && L > 0, "ln_tab_prep: bad arguments");
   F5_CHECK_CUDA(launch_kernel(ln_tab_prep_kernel, dim3(T, 2 * L + 1), dim3(256), 0, st, mod,
                               reinterpret_cast<__nv_bfloat16*>(prep_bf16), T, L, D, NM));
@@ -54,7 +54,7 @@ int launch_ln_tab_prep(const float* mod, void* prep_bf16, int T, int L, int D, i
 
 int launch_dwconv7_ln(const float* x, void* y, int B, int N, int C, const float* wt,
                       const float* wb, const float* ln_w, const float* ln_b, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(x && y && wt && wb && ln_w && ln_b, "dwconv7_ln: null pointer");
   const int blocks = cdiv(B * N * 32, 256);
   __nv_bfloat16* yo = reinterpret_cast<__nv_bfloat16*>(y);
@@ -70,7 +70,7 @@ int launch_dwconv7_ln(const float* x, void* y, int B, int N, int C, const float*
 
 int launch_grn(const void* h, void* y, float* nx_scratch, const float* gamma, const float* beta,
                int B, int N, int C, cudaStream_t st, const int* valid_len) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(h && y && nx_scratch && gamma && beta, "grn: null pointer");
   F5_REQUIRE(C % 4 == 0, "grn: C %% 4");
   const int nblk = cdiv(N, kGrnRowsPerBlock);
@@ -89,7 +89,7 @@ int launch_grn(const void* h, void* y, float* nx_scratch, const float* gamma, co
 int launch_text_embed_gather(const int* text, int B, int nt, int N, int C, const float* emb,
                              const float* pos_table, int max_pos, float* x, int Bout,
                              int drop_from, cudaStream_t st, int mask_padding, const int* valid_len) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(text && emb && pos_table && x, "text_embed_gather: null pointer");
   F5_REQUIRE(C % 4 == 0, "text_embed_gather: C %% 4");
   F5_CHECK_CUDA(launch_kernel(text_embed_gather_kernel, dim3(dim3(N, Bout)), dim3(128), 0, st, text, B, nt, N, C, emb, pos_table,
@@ -101,7 +101,7 @@ int launch_text_embed_gather(const int* text, int B, int nt, int N, int C, const
 int launch_time_mlp(const float* tvals, int T, int D, const float* w0, const float* b0,
                     const float* w2, const float* b2, float* t_emb, void* silu_bf16,
                     cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(tvals && w0 && b0 && w2 && b2 && silu_bf16, "time_mlp: null pointer");
   F5_CHECK_CUDA(launch_kernel(time_mlp_kernel, dim3(T, cdiv(D, kTimeMlpCols)), dim3(256), (256 + D) * sizeof(float), st, 
       tvals, D, w0, b0, w2, b2, t_emb, reinterpret_cast<__nv_bfloat16*>(silu_bf16)));
@@ -110,7 +110,7 @@ int launch_time_mlp(const float* tvals, int T, int D, const float* w0, const flo
 }
 
 int launch_ode_update(const OdeUpdateParams& p, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   const long long tot = (long long)p.rows * p.d;
   F5_CHECK_CUDA(launch_kernel(cfg_ode_update_kernel, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, p));
   F5_CHECK_CUDA(cudaGetLastError());
@@ -119,7 +119,7 @@ int launch_ode_update(const OdeUpdateParams& p, cudaStream_t st) {
 
 int launch_cast_pad_bf16(const float* src, int d, void* dst, int ld, int rows,
                          long long copy_row_offset, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   const long long tot = (long long)rows * ld;
   F5_CHECK_CUDA(launch_kernel(cast_pad_bf16_kernel, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, 
       src, d, reinterpret_cast<__nv_bfloat16*>(dst), ld, rows, copy_row_offset));
@@ -130,7 +130,7 @@ int launch_cast_pad_bf16(const float* src, int d, void* dst, int ld, int rows,
 int launch_concat_cond_text(const float* cond, int dc, int Bc, int N, const float* text, int dt,
                             void* dst, int ld, int rows, int drop_from_row, cudaStream_t st,
                             const int* cond_len) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   const long long tot = (long long)rows * ld;
   F5_CHECK_CUDA(launch_kernel(concat_cond_text_kernel, dim3((unsigned)((tot + 255) / 256)), dim3(256), 0, st, 
       cond, dc, Bc, N, text, dt, reinterpret_cast<__nv_bfloat16*>(dst), ld, rows, drop_from_row, cond_len));
@@ -140,7 +140,7 @@ int launch_concat_cond_text(const float* cond, int dc, int Bc, int N, const floa
 
 int launch_duration_head(const float* x, int B, int N, int D, const int* len, const float* norm_w,
                          const float* pred_w, float* out, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0, st);
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
   F5_REQUIRE(x && len && norm_w && pred_w && out, "duration_head: null pointer");
   switch (D) {
     case 256: F5_CHECK_CUDA(launch_kernel(duration_head_kernel<256>, dim3(B), dim3(256), 0, st, x, N, len, norm_w, pred_w, out)); break;

@@ -1,6 +1,4 @@
 // Host launcher + C-ABI entry for the wgmma GEMM (see gemm_sm90.cuh and include/f5_b200.h).
-#include <stdlib.h>
-
 #include "gemm_sm90.cuh"
 #include "host_common.h"
 
@@ -16,8 +14,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   const double taps = p.conv_taps;
   ProfScope ps(PROF_GEMM, 2.0 * p.M * (double)p.N * (double)p.k_per_tap * taps,
                2.0 * ((double)p.M * p.k_per_tap + (double)p.N * p.k_per_tap * taps) +
-                   (double)p.M * p.N * (OUT_BF16 ? 2.0 : 4.0),
-               stream);
+                   (double)p.M * p.N * (OUT_BF16 ? 2.0 : 4.0));
   GemmParams q = p;
   q.prof = ps.slot;
   F5_CHECK_CUDA(launch_kernel(kern, dim3(grid), dim3(GemmEpi<BN>::kThreads), S::kTotal, stream, ta, tb, to, to2, q));
@@ -81,27 +78,9 @@ static int dispatch_scaled(int act, bool out_bf16, bool rope, const CUtensorMap&
 
 }  // namespace f5
 
-// Debug aid: give successive f5_gemm_bf16 calls consecutive slices of a timestamp buffer, so the
-// per-CTA phase timelines of every GEMM of a (graph-captured) step can be read back in situ.
-static char* g_ts_base = nullptr;
-static long long g_ts_stride = 0;
-static int g_ts_max = 0, g_ts_idx = 0;
-extern "C" int f5_debug_gemm_ts(void* base, int64_t stride_bytes, int32_t max_calls) {
-  g_ts_base = reinterpret_cast<char*>(base);
-  g_ts_stride = stride_bytes;
-  g_ts_max = max_calls;
-  g_ts_idx = 0;
-  return 0;
-}
-
-extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
+extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   using namespace f5;
   if (int e = device_check()) return e;
-  F5_REQUIRE(a_in != nullptr, "f5_gemm_bf16: null args");
-  f5_gemm_args a_copy = *a_in;
-  if (g_ts_base && g_ts_idx < g_ts_max && a_copy.debug_ts == nullptr)
-    a_copy.debug_ts = g_ts_base + (long long)(g_ts_idx++) * g_ts_stride;
-  const f5_gemm_args* a = &a_copy;
   F5_REQUIRE(a != nullptr, "f5_gemm_bf16: null args");
   F5_REQUIRE(a->a && a->w && a->out, "f5_gemm_bf16: null operand pointer");
   F5_REQUIRE(a->m > 0 && a->n > 0 && a->k > 0, "f5_gemm_bf16: bad shape m=%d n=%d k=%d", a->m,
@@ -145,7 +124,6 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   if (a->out2_scale)
     F5_REQUIRE(a->out2_bf16 && a->out2_fp8 && a->n % 64 == 0, "f5_gemm_bf16: out2_scale needs an e4m3 out2 and n %% 64 == 0");
   if (a->resid) F5_REQUIRE(a->ldr % 4 == 0, "f5_gemm_bf16: ldr not multiple of 4");
-  if (a->gate) F5_REQUIRE(a->gate_ld % 4 == 0, "f5_gemm_bf16: gate_ld not multiple of 4");
 
   // output tensor maps (TMA stores of the epilogue): (cols, rows per utterance, utterances) when tiles never straddle
   // utterances, else (cols, m, 1)
@@ -162,12 +140,9 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
     }
   }
 
-  // tile width: 64 or 128 columns.  `variant` selects nothing on sm_90 (there is one kernel family); wider tile
-  // requests (192, 256) get the widest tile there is.
-  F5_REQUIRE(a->variant >= 0 && a->variant <= 2, "f5_gemm_bf16: variant must be 0, 1 or 2");
-  F5_REQUIRE(a->tile_n == 0 || a->tile_n == 64 || a->tile_n == 128 || a->tile_n == 192 || a->tile_n == 256,
-             "f5_gemm_bf16: tile_n must be 0, 64, 128, 192 or 256");
-  int bn = a->tile_n > 128 ? 128 : a->tile_n;
+  // tile width: 64 or 128 columns
+  F5_REQUIRE(a->tile_n == 0 || a->tile_n == 64 || a->tile_n == 128, "f5_gemm_bf16: tile_n must be 0, 64 or 128");
+  int bn = a->tile_n;
   if (a->conv_grouped) bn = 64;
   if (bn == 0) {
     // fill the SMs: prefer 128-wide tiles unless that leaves most SMs idle
@@ -188,7 +163,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   p.bias = a->bias;
   p.out = a->out; p.ldo = (int)a->ldo;
   p.resid = a->resid; p.ldr = (int)a->ldr;
-  p.gate = a->gate; p.gate_ld = (int)a->gate_ld;
+  p.gate = a->gate;
   p.row_len = a->row_len;
   p.rope = reinterpret_cast<const float2*>(a->rope);
   p.rope_cols = a->rope_cols;
@@ -196,7 +171,6 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a_in, void* stream_) {
   p.q_cols = a->q_cols;
   p.out2 = reinterpret_cast<__nv_bfloat16*>(a->out2_bf16);
   p.ldo2 = (int)a->ldo2;
-  p.ts = reinterpret_cast<unsigned long long*>(a->debug_ts);
   p.w_static = a->w_static;
   p.pf_ptr = reinterpret_cast<const char*>(a->prefetch); p.pf_bytes = a->prefetch_bytes;
   p.ln_scale = a->ln_scale; p.ln_stats = reinterpret_cast<float2*>(a->ln_stats);

@@ -24,8 +24,7 @@ struct GemmParams {
   int ldo;
   const float* resid;      // f32 [rows, ldr] or null (may alias out)
   int ldr;
-  const float* gate;       // f32 [num_batches, gate_ld] or null
-  int gate_ld;
+  const float* gate;       // f32 [N], shared by all utterances, or null
   const int* row_len;      // [num_batches] valid frames per utterance, or null
   const float2* rope;      // [rows_per_batch, 32] (cos, sin), or null
   int rope_cols;
@@ -33,7 +32,6 @@ struct GemmParams {
   int q_cols;
   __nv_bfloat16* out2;     // optional bf16 copy of the result
   int ldo2;
-  unsigned long long* ts;  // debug: per-CTA phase timestamps (globaltimer ns), 10 slots per CTA, or null
   unsigned long long* prof;  // in-graph timing slot (ptx.cuh prof_stamp_*), or null
   int w_static;            // B operand may be fetched before the PDL wait (weights)
   const char* pf_ptr;      // weights of a LATER GEMM to pull into L2 while this one runs, or null
@@ -74,14 +72,6 @@ __device__ __forceinline__ void prefetch_slice_l2(const GemmParams& p, int cta, 
     asm volatile("prefetch.global.L2 [%0];" ::"l"(p.pf_ptr + o));
 }
 
-__device__ __forceinline__ void ts_mark(const GemmParams& p, int cta, int slot) {
-  if (p.ts != nullptr) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    p.ts[(size_t)cta * 10 + slot] = t;
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // Epilogue, organised for memory-level parallelism (a load -> use chain per operand and chunk leaves the
 // epilogue latency-bound):
@@ -108,8 +98,8 @@ __device__ __forceinline__ float mish_fast(float x) {
   return x * tanh_approx(sp);
 }
 
-// stage bias[n0..n0+BN) and gate[n0..n0+BN) (gate only when it is shared by all utterances,
-// gate_ld == 0) into shared memory; called by the 128 epilogue threads, `et` = 0..127
+// stage bias[n0..n0+BN) and gate[n0..n0+BN) (1 when there is no gate) into shared memory; called by the 128 epilogue
+// threads, `et` = 0..127
 // aux_s: c1 of the fused-LN consumer mode, or the second output's scale 1 + ln_scale (1 when there is none) — a GEMM is
 // never both.  In consumer mode bias_s holds c2 + bias.
 // ws_s (SCALED instantiations): acc_scale * w_scale[col], the factor of the accumulator term.
@@ -129,7 +119,7 @@ __device__ __forceinline__ void epi_stage_cols(const GemmParams& p, int n0, int 
       b += t[2 * p.ln_tab_ld] + t[3 * p.ln_tab_ld];
     }
     bias_s[i] = b;
-    gate_s[i] = (p.gate != nullptr && p.gate_ld == 0 && ok) ? p.gate[col] : 1.f;
+    gate_s[i] = (p.gate != nullptr && ok) ? p.gate[col] : 1.f;
     aux_s[i] = x;
   }
 }
@@ -352,7 +342,7 @@ template <int ACT, bool OUT_BF16, bool ROPE, int HALF, bool SC = false>
 __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float4 (&res)[8],
                                           const float* bias_s, const float* gate_s, const float* aux_s,
                                           const float2 (&cs)[ROPE ? 32 : 1], const GemmParams& p,
-                                          int col0, int row, int b_idx, bool row_ok, bool row_valid,
+                                          int col0, int row, bool row_ok, bool row_valid,
                                           const EpiStage& st, float2& unit_acc, const float* ws_s = nullptr,
                                           float* unit_amax = nullptr) {
   float v[32];
@@ -423,24 +413,12 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
       for (int j = 0; j < 32; ++j) v[j] = 0.f;
     }
   }
-  if (p.gate != nullptr && p.gate_ld == 0) {     // residual + gate * v as one FMA per element
+  // residual + gate * v as one FMA per element; without a gate gate_s is 1, and fmaf(v, 1, r) rounds exactly as v + r
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float4 gg = *reinterpret_cast<const float4*>(gate_s + 4 * j);
-      v[4 * j] = fmaf(v[4 * j], gg.x, res[j].x); v[4 * j + 1] = fmaf(v[4 * j + 1], gg.y, res[j].y);
-      v[4 * j + 2] = fmaf(v[4 * j + 2], gg.z, res[j].z); v[4 * j + 3] = fmaf(v[4 * j + 3], gg.w, res[j].w);
-    }
-  } else {
-    if (p.gate != nullptr) {   // per-utterance gates (not used by sample(): all utterances share the time value)
-      const float* g = p.gate + (size_t)b_idx * p.gate_ld + col0;
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col0 + j < p.N) v[j] *= g[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      v[4 * j] += res[j].x; v[4 * j + 1] += res[j].y; v[4 * j + 2] += res[j].z; v[4 * j + 3] += res[j].w;
-    }
+  for (int j = 0; j < 8; ++j) {
+    const float4 gg = *reinterpret_cast<const float4*>(gate_s + 4 * j);
+    v[4 * j] = fmaf(v[4 * j], gg.x, res[j].x); v[4 * j + 1] = fmaf(v[4 * j + 1], gg.y, res[j].y);
+    v[4 * j + 2] = fmaf(v[4 * j + 2], gg.z, res[j].z); v[4 * j + 3] = fmaf(v[4 * j + 3], gg.w, res[j].w);
   }
   if constexpr (!OUT_BF16) {
     if (p.out2 != nullptr) {
@@ -530,7 +508,7 @@ template <int BN, int ACT, bool OUT_BF16, bool ROPE, bool SC = false>
 __device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float* bias_s,
                                                const float* gate_s, const float* aux_s, const float2 (&cs)[ROPE ? 32 : 1],
                                                float4 (&res0)[8], const GemmParams& p, int n0, int row,
-                                               int b_idx, bool row_ok, bool row_valid, EpiStage& st,
+                                               bool row_ok, bool row_valid, EpiStage& st,
                                                const float* ws_s = nullptr) {
   float4 res1[8];
   float2 unit_acc = make_float2(0.f, 0.f);
@@ -545,14 +523,13 @@ __device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float
     acc_ld32(acc_row + cc * 64, acc);
     if (colA < p.N)   // uniform per CTA
       epi_apply<ACT, OUT_BF16, ROPE, 0, SC>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
-                                            b_idx, row_ok, row_valid, st, unit_acc, SC ? ws_s + cc * 64 : nullptr,
-                                            &unit_amax);
+                                            row_ok, row_valid, st, unit_acc, SC ? ws_s + cc * 64 : nullptr, &unit_amax);
     // chunk B: request the next unit's first residual, then drain B
     if (cc + 1 < BN / 64) epi_load_resid(p, row, colA + 64, row_ok, res0);
     acc_ld32(acc_row + cc * 64 + 32, acc);
     if (colB < p.N)
       epi_apply<ACT, OUT_BF16, ROPE, 1, SC>(acc, res1, bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs,
-                                            p, colB, row, b_idx, row_ok, row_valid, st, unit_acc,
+                                            p, colB, row, row_ok, row_valid, st, unit_acc,
                                             SC ? ws_s + cc * 64 + 32 : nullptr, &unit_amax);
   }
 }

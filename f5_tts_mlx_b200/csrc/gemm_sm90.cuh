@@ -20,8 +20,7 @@
 //   RoPE on adjacent column pairs for col < rope_cols     (rope.py:87-107, dit.py:157-158)
 //   v *= q_scale for col < q_cols                         softmax scale folded into q (dit.py:166)
 //   v = row valid ? v : 0                                 "x * mask" (dit.py:172-173)
-//   v *= gate[batch, col]                                 AdaLN-Zero gate (dit.py:319,323)
-//   v += resid[row, col]                                  residual (fp32 stream)
+//   v = v * gate[col] + resid[row, col]                   AdaLN-Zero gate (dit.py:319,323), residual (fp32 stream)
 //   store fp32 or bf16
 #pragma once
 #include <type_traits>
@@ -112,8 +111,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
 
   // ---- one-time setup (overlaps the predecessor kernel under PDL) ----
   const int cta_lin = blockIdx.y * gridDim.x + blockIdx.x;
-  if (threadIdx.x == 0) ts_mark(p, cta_lin, 0);
-  if (warp == 0 && F5_ELECT_LANE()) {
+  if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
     tma_prefetch_desc(&tma_out);
@@ -126,25 +124,24 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
   }
   if (warp == 1) prefetch_slice_l2(p, cta_lin, gridDim.x * gridDim.y, lane);
   __syncthreads();
-  if (threadIdx.x == 0) ts_mark(p, cta_lin, 1);
   // weights do not depend on the predecessor kernel: the first ring of B tiles is requested BEFORE the PDL
   // wait, so their (possibly HBM) latency runs under the predecessor's tail
   const int early_b = p.w_static ? min(kStages, num_kb) : 0;
-  if (warp == 0 && F5_ELECT_LANE()) {
+  if (warp == 0 && elect_one()) {
     for (int kb = 0; kb < early_b; ++kb) {
       mbar_expect_tx(&full_bar[kb], S::kStageBytes);
       tma_load_2d(smem + kb * S::kStageBytes + S::kABytes, &tma_b, &full_bar[kb], kb * kbe, n0);
     }
   }
   pdl_wait();   // predecessor's outputs (our A operand / residual) are complete and visible
-  if (threadIdx.x == 128) { ts_mark(p, cta_lin, 2); prof_stamp_begin(p.prof); }
+  if (threadIdx.x == 128) prof_stamp_begin(p.prof);
 
   // Registers move from the producer warpgroup (one thread issues TMA) to the consumers, whose epilogue holds RoPE
   // tables and residual tiles next to the accumulator chunk: 128 x 40 + 256 x 232 = the 384 x 168 of the launch.
   if (warp < 4) {
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-    if (warp == 0 && F5_ELECT_LANE()) {
+    if (warp == 0 && elect_one()) {
       auto produce = [&](auto ab8_tag) {
         constexpr int KBE = decltype(ab8_tag)::value ? 128 : 64;     // elements per k-block, compile-time in the loop
         // incremental stage / phase / tap bookkeeping: no division in the loop
@@ -294,7 +291,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
     pdl_launch_dependents();
     if (grp < E::kGroups) {
       // ===================== epilogue =====================
-      if (et == 0 && grp == 0) ts_mark(p, cta_lin, 7);
       const int r_in_tile = et;
       const int m_in_batch = m_in_batch0 + r_in_tile;
       const int row = row0 + r_in_tile;
@@ -334,14 +330,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
       stg.mu_r = ln_mu_r; stg.rstd = ln_rstd;
       stg.out_fp8 = p.out_fp8;
       epi_drain_tile<BNG, ACT, OUT_BF16, ROPE, SCALED>(acc_s + r_in_tile * S::kAccLd + grp * BNG, bias_s, gate_s, aux_s,
-                                                       cs, res0, p, n0g, row, b_idx, row_ok, row_valid, stg, ws_s);
+                                                       cs, res0, p, n0g, row, row_ok, row_valid, stg, ws_s);
       if (et == 0) tma_store_wait_read<0>();   // the staging buffers must outlive the TMA unit's reads; grid completion
                                                // makes the global writes visible to the dependent kernel
     }
   }
 
   __syncthreads();
-  if (threadIdx.x == 0) { ts_mark(p, cta_lin, 9); prof_stamp_end(p.prof); }
+  if (threadIdx.x == 0) prof_stamp_end(p.prof);
 }
 
 }  // namespace f5

@@ -1,7 +1,5 @@
 #include "host_common.h"
 
-#include <stdlib.h>
-
 #include <atomic>
 #include <mutex>
 #include <vector>
@@ -16,17 +14,6 @@ int set_error(int code, const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
   return code;
-}
-
-bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    // the trigger sits at the start of each kernel's epilogue (a trigger at kernel start makes the dependent
-    // grid resident too early and takes SMs from the running one).  F5_PDL=0 disables.
-    const char* v = getenv("F5_PDL");
-    on = (v && v[0] == '0') ? 0 : 1;
-  }
-  return on != 0;
 }
 
 int sm_count() {
@@ -143,19 +130,16 @@ int make_tmap_out(CUtensorMap* map, const void* base, int elem_bytes, uint64_t c
 }
 
 // ---------------------------------------------------------------------------------------------
-// launch accounting / profiling
+// launch accounting / in-graph timing
 // ---------------------------------------------------------------------------------------------
-struct ProfRec { int kind; double flops, bytes; cudaEvent_t e0, e1; };
 static std::mutex g_prof_mu;
-static bool g_prof_on = false;
-static std::vector<ProfRec> g_prof;
 static std::atomic<long long> g_launches{0};
 struct GraphSlotMeta { int kind; double flops, bytes; };
 static unsigned long long* g_gslots = nullptr;
 static int g_gslots_cap = 0;
 static std::vector<GraphSlotMeta> g_gmeta;
 
-ProfScope::ProfScope(int kind, double flops, double bytes, cudaStream_t st) : idx_(-1), st_(st), slot(nullptr) {
+ProfScope::ProfScope(int kind, double flops, double bytes) : slot(nullptr) {
   g_launches.fetch_add(1, std::memory_order_relaxed);
   if (g_gslots != nullptr) {
     std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -164,32 +148,12 @@ ProfScope::ProfScope(int kind, double flops, double bytes, cudaStream_t st) : id
       g_gmeta.push_back({kind, flops, bytes});
     }
   }
-  if (!g_prof_on) return;
-  std::lock_guard<std::mutex> lk(g_prof_mu);
-  ProfRec r;
-  r.kind = kind; r.flops = flops; r.bytes = bytes;
-  if (cudaEventCreate(&r.e0) != cudaSuccess || cudaEventCreate(&r.e1) != cudaSuccess) return;
-  cudaEventRecord(r.e0, st);
-  g_prof.push_back(r);
-  idx_ = (int)g_prof.size() - 1;
-}
-ProfScope::~ProfScope() {
-  if (idx_ < 0) return;
-  std::lock_guard<std::mutex> lk(g_prof_mu);
-  cudaEventRecord(g_prof[idx_].e1, st_);
 }
 
 }  // namespace f5
 
 extern "C" {
 long long f5_launch_count(void) { return f5::g_launches.load(); }
-int f5_prof_enable(int on) {
-  std::lock_guard<std::mutex> lk(f5::g_prof_mu);
-  for (auto& r : f5::g_prof) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
-  f5::g_prof.clear();
-  f5::g_prof_on = on != 0;
-  return 0;
-}
 // In-graph timing: install a device buffer of `max_slots` x 2 uint64 (the caller fills [*,0] with UINT64_MAX and
 // [*,1] with 0 before each run); slot i belongs to the i-th ProfScope opened from now on.  NULL uninstalls.
 int f5_prof_graph_begin(void* slots, int32_t max_slots) {
@@ -211,22 +175,6 @@ int f5_prof_graph_meta(int32_t* kinds, double* flops, double* bytes, int32_t cap
   }
   return n;
 }
-// out: [kinds][4] = {milliseconds, flops, bytes, launches}
-int f5_prof_summary(double* out, int kinds) {
-  std::lock_guard<std::mutex> lk(f5::g_prof_mu);
-  for (int i = 0; i < kinds * 4; ++i) out[i] = 0.0;
-  for (auto& r : f5::g_prof) {
-    if (r.kind >= kinds) continue;
-    if (cudaEventSynchronize(r.e1) != cudaSuccess) return f5::set_error(F5_ERR_CUDA, "prof: event sync failed");
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, r.e0, r.e1);
-    out[r.kind * 4 + 0] += ms;
-    out[r.kind * 4 + 1] += r.flops;
-    out[r.kind * 4 + 2] += r.bytes;
-    out[r.kind * 4 + 3] += 1.0;
-  }
-  return 0;
-}
 // sizeof() of every struct of the ABI, so a binding can verify its own layout at load time
 int f5_struct_sizes(int32_t* out, int32_t n) {
   const int32_t v[10] = {(int32_t)sizeof(f5_gemm_args),          (int32_t)sizeof(f5_convnext_weights),
@@ -238,6 +186,6 @@ int f5_struct_sizes(int32_t* out, int32_t n) {
   return 10;
 }
 const char* f5_last_error(void) { return f5::g_err; }
-int f5_abi_version(void) { return 1102; }
+int f5_abi_version(void) { return 2000; }
 int f5_device_check(void) { return f5::device_check(); }
 }

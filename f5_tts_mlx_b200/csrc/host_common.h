@@ -47,8 +47,7 @@ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 // SM count of the CURRENT device (cached per device: one process may drive several GPUs)
 int sm_count();
 
-// Launch with the programmatic-dependent-launch attribute (see ptx.cuh); F5_PDL=0 disables it.
-bool pdl_enabled();
+// Launch with the programmatic-dependent-launch attribute (see ptx.cuh).
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
                                  cudaStream_t st, Args&&... args) {
@@ -61,7 +60,7 @@ inline cudaError_t launch_kernel(void (*kern)(KArgs...), dim3 grid, dim3 block, 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
@@ -81,19 +80,14 @@ inline cudaError_t ensure_dyn_smem(SmemAttrOnce& once, K kern, int bytes) {
   return e;
 }
 
-// ---- launch accounting + optional per-kernel-family device timing (bench.py roofline) ----
-// Every launcher opens a ProfScope around its kernel launch.  The launch counter is always on;
-// when profiling is enabled (f5_prof_enable) a CUDA event pair brackets the launch on its stream
-// and f5_prof_summary returns the summed device time / algorithmic FLOPs / bytes per family.
+// ---- launch accounting + in-graph per-kernel timing (bench.py roofline) ----
+// Every launcher opens a ProfScope before its kernel launch, which counts the launch (f5_launch_count).
 enum ProfKind { PROF_GEMM = 0, PROF_ATTN = 1, PROF_LN = 2, PROF_OTHER = 3, PROF_NKINDS = 4 };
 // In-graph timing (f5_prof_graph_begin): while a slot buffer is installed every ProfScope also hands its kernel one
 // slot of two uint64 — [0] atomicMin(globaltimer) when a CTA has passed its dependency wait, [1] atomicMax at CTA
 // exit — whose address is baked into a captured CUDA graph, so one replay yields every kernel's in-situ duration.
 struct ProfScope {
-  ProfScope(int kind, double flops, double bytes, cudaStream_t st);
-  ~ProfScope();
-  int idx_;
-  cudaStream_t st_;
+  ProfScope(int kind, double flops, double bytes);
   unsigned long long* slot;   // device pointer or nullptr
 };
 

@@ -19,6 +19,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// One thread of a CONVERGED warp.  Choosing it with elect.sync instead of `lane == 0` keeps the single-thread TMA
+// loops free of the compiler's per-instruction serialisation loop around uniform-datapath operations.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -28,17 +30,6 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-// One thread of a CONVERGED warp.  Choosing it with elect.sync instead of `lane == 0` keeps the single-thread TMA
-// loops free of the compiler's per-instruction serialisation loop around uniform-datapath operations.
-// F5_ELECT_MODE=0 restores lane 0 for A/B measurements.
-#ifndef F5_ELECT_MODE
-#define F5_ELECT_MODE 1
-#endif
-#if F5_ELECT_MODE
-#define F5_ELECT_LANE() ::f5::elect_one()
-#else
-#define F5_ELECT_LANE() (lane == 0)
-#endif
 
 // ---------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization

@@ -40,7 +40,7 @@ def gemm(
     bias: torch.Tensor | None = None,
     act: int = ACT_NONE,
     resid: torch.Tensor | None = None,
-    gate: torch.Tensor | None = None,      # f32 [num_batches, n] view (row stride honoured)
+    gate: torch.Tensor | None = None,      # f32 [n], shared by all utterances: out = v * gate + resid
     row_len: torch.Tensor | None = None,   # i32 [num_batches]
     rope: torch.Tensor | None = None,      # f32 [rows_per_batch, 32, 2]
     rope_cols: int = 0,
@@ -52,9 +52,7 @@ def gemm(
     conv_taps: int = 1,
     conv_pad: int = 0,
     conv_grouped: bool = False,
-    tile_n: int = 0,
-    variant: int = 0,
-    debug_ts: torch.Tensor | None = None,
+    tile_n: int = 0,                       # 0 (auto), 64 or 128
     out2: torch.Tensor | None = None,          # bf16 [rows, >=n] second copy (or the fused-LN operand, see ln_scale)
     ln_scale: torch.Tensor | None = None,      # f32 [n]: producer mode — out2 = bf16(out * (1 + ln_scale)), ln_stats filled
     ln_stats: torch.Tensor | None = None,      # f32 [rows, n/64, 2] (sum, sum of squares) per 64 columns
@@ -101,8 +99,8 @@ def gemm(
         assert resid.dtype == torch.float32
         g.resid, g.ldr = resid.data_ptr(), resid.stride(0)
     if gate is not None:
-        assert gate.dtype == torch.float32 and gate.stride(-1) == 1
-        g.gate, g.gate_ld = gate.data_ptr(), gate.stride(0) if gate.dim() > 1 else 0
+        assert gate.dtype == torch.float32 and gate.dim() == 1 and gate.stride(-1) == 1
+        g.gate = gate.data_ptr()
     if row_len is not None:
         assert row_len.dtype == torch.int32
         g.row_len = row_len.data_ptr()
@@ -111,9 +109,6 @@ def gemm(
         g.rope = rope.data_ptr()
     g.rope_cols, g.q_scale, g.q_cols = rope_cols, q_scale, q_cols
     g.tile_n = tile_n
-    g.variant = variant
-    if debug_ts is not None:
-        g.debug_ts = debug_ts.data_ptr()
     g.ab_fp8, g.acc_scale, g.out2_fp8 = int(ab_fp8), float(acc_scale), int(out2_fp8)
     g.w_static = int(w_static)
     if prefetch is not None:

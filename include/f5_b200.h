@@ -40,21 +40,17 @@ int f5_abi_version(void);
 int f5_device_check(void);
 /* number of kernels this library has launched in this process (bench.py "gpu_launches") */
 long long f5_launch_count(void);
-/* optional per-kernel-family device timing: enable, run, then read
- * out[kinds][4] = {milliseconds, algorithmic flops, bytes, launches}; kinds: 0 GEMM, 1 attention,
- * 2 LayerNorm+modulate, 3 everything else. */
 /* sizeof() of the ABI structs in declaration order: f5_gemm_args, f5_convnext_weights,
  * f5_dit_block_weights, f5_dit_weights, f5_dit_buffers, f5_vocos_block_weights, f5_vocos_weights,
  * f5_vocos_buffers, f5_duration_weights, f5_duration_buffers — lets a binding check its layout at
  * load time.  Returns the count (10). */
 int f5_struct_sizes(int32_t* out, int32_t n);
-int f5_prof_enable(int on);
-int f5_prof_summary(double* out, int kinds);
 /* In-situ kernel timing inside a captured CUDA graph (bench.py's roofline): install a device buffer of max_slots x 2
  * uint64; from then on the i-th launched kernel of the tensor-core families (GEMM, attention) gets slot i and writes
  * [i][0] = min over its CTAs of %globaltimer after the dependency wait, [i][1] = max over CTAs at exit (the caller
- * presets the columns to UINT64_MAX / 0 before each replay).  f5_prof_graph_meta returns the family (kinds as above)
- * and the algorithmic flops / bytes of every slot handed out since the install; slots = NULL uninstalls. */
+ * presets the columns to UINT64_MAX / 0 before each replay).  f5_prof_graph_meta returns the family of every slot
+ * handed out since the install (0 GEMM, 1 attention, 2 LayerNorm+modulate, 3 everything else) and its algorithmic
+ * flops / bytes; slots = NULL uninstalls. */
 int f5_prof_graph_begin(void* slots, int32_t max_slots);
 int f5_prof_graph_meta(int32_t* kinds, double* flops, double* bytes, int32_t cap);
 
@@ -91,21 +87,18 @@ typedef struct f5_gemm_args {
   int64_t ldo;
   const float* resid;     /* fp32 [rows, ldr] or NULL; may alias out                            */
   int64_t ldr;
-  const float* gate;      /* fp32 [num_batches, gate_ld] or NULL                                */
-  int64_t gate_ld;
+  const float* gate;      /* fp32 [n], shared by all utterances, or NULL: out = v * gate + resid */
   const int32_t* row_len; /* [num_batches] valid frames (rows beyond are written as 0) or NULL  */
   const float* rope;      /* fp32 [rows_per_batch, 32, 2] (cos,sin) or NULL                     */
   int32_t rope_cols;      /* columns [0, rope_cols) are rotated in adjacent pairs               */
   float q_scale;          /* columns [0, q_cols) are multiplied by q_scale after the rotation   */
   int32_t q_cols;
-  int32_t tile_n;         /* 0 = auto, else 64 | 128 (192 | 256 are accepted and run as 128)     */
+  int32_t tile_n;         /* 0 = auto, else 64 | 128                                             */
   void* out2_bf16;        /* optional second copy of the result as bf16 [rows, ldo2], or NULL    */
   int64_t ldo2;
-  int32_t variant;        /* 0 | 1 | 2, kept for ABI compatibility: sm_90 has one 128xBN kernel   */
   int32_t w_static;       /* nonzero: `w` is never written by work that precedes this call on the stream
                              (model weights): the kernel may start fetching it before its programmatic
                              dependency on the preceding kernel has resolved                           */
-  void* debug_ts;         /* NULL, or uint64 [ctas, 10]: per-CTA phase timestamps (globaltimer ns)  */
   const void* prefetch;   /* NULL, or device memory (weights of a later GEMM) to pull into L2       */
   int64_t prefetch_bytes;
   /* Fused AdaLayerNormZero (dit.py:262-271, 281-290; call sites dit.py:313,321,397) by linearity of the Linear that
@@ -147,9 +140,6 @@ typedef struct f5_gemm_args {
 } f5_gemm_args;
 
 int f5_gemm_bf16(const f5_gemm_args* args, void* stream);
-/* debug aid: the next `max_calls` f5_gemm_bf16 calls without their own debug_ts write their per-CTA
- * timestamps to base + i * stride_bytes (i = call index); pass NULL to stop. */
-int f5_debug_gemm_ts(void* base, int64_t stride_bytes, int32_t max_calls);
 
 /* ------------------------------------------------------------------------------------------ *
  * Flash-attention forward (non-causal, key-padding mask, head_dim 64) — replaces
@@ -170,8 +160,6 @@ int f5_attention_fwd_e4m3(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
 int f5_attention_fwd_e4m3_scaled(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch,
                                  int32_t frames, int32_t heads, int32_t head_dim, const int32_t* kv_len,
                                  float* scale_out, void* stream);
-/* kept for ABI compatibility: accepts any `base` and returns 0; the attention kernel records no timeline */
-int f5_debug_attention_ts(void* base);
 
 /* ------------------------------------------------------------------------------------------ *
  * HBM-bound pieces.
@@ -261,14 +249,16 @@ typedef struct f5_dit_block_weights {
   const void* out_w;  const float* out_b;   /* [D, D]                     (dit.py:124)     */
   const void* ff1_w;  const float* ff1_b;   /* [F, D]                     (dit.py:94-95)   */
   const void* ff2_w;  const float* ff2_b;   /* [D, F]                     (dit.py:96)      */
-  /* FP8 mode (optional, NULL = bf16 only): e4m3 copies of the QKV / FF1 weights, ONE scale per tensor
-   * (w ~= scale * e4m3); used by f5_dit_forward when f5_dit_buffers.a_fp8 is set (see f5_gemm_args.ab_fp8).  With
-   * out_w8 / ff2_w8 also the out-projection (attention writes e4m3) and FF2 (FF1 writes e4m3) run in FP8. */
+  /* FP8 mode (optional, NULL = bf16 only): e4m3 copies of the four block weights, ONE scale per tensor
+   * (w ~= scale * e4m3); used by f5_dit_forward when f5_dit_buffers.a_fp8 is set (see f5_gemm_args.ab_fp8), which then
+   * needs all four in every block.  All four block GEMMs run in FP8: the attention and FF1 write e4m3 for the
+   * out-projection and FF2. */
   const void* qkv_w8; const void* ff1_w8; const void* out_w8; const void* ff2_w8;
   float qkv_s8, ff1_s8, out_s8, ff2_s8;
   /* Block-scaled FP8 mode (ABI 1.101, optional): fp32 per-output-channel scales of the *_w8 weights (w[o] ~= s[o] *
    * e4m3, *_s8 = 1).  With these and f5_dit_buffers.a_fp8 / a_fp8_scale / attn_scale / ff_scale all set, the four block
-   * GEMMs run on block-scaled e4m3 operands (see f5_gemm_args.a_scale). */
+   * GEMMs run on block-scaled e4m3 operands (see f5_gemm_args.a_scale).  In FP8 mode they need the block-scale buffers:
+   * all four in every block, or none. */
   const float* qkv_ws; const float* ff1_ws; const float* out_ws; const float* ff2_ws;
 } f5_dit_block_weights;
 
@@ -326,8 +316,9 @@ typedef struct f5_dit_buffers {
   void* qkv_bf16;             /* bf16 [rows, 3D] */
   void* ff_bf16;              /* bf16 [rows, ff_inner] */
   float* v;                   /* fp32 [rows, mel_dim]: DiT output (flow prediction) */
-  /* Fused AdaLN (see f5_gemm_args.ln_*): all three non-NULL selects it, any NULL keeps the separate
-   * f5_ln_modulate launches.  ln_tab_ld = depth*(3D + ff_inner) + 128 (f5_dit_ln_tab_ld). */
+  /* Fused AdaLN (see f5_gemm_args.ln_*): all three set selects it, all three NULL keeps the separate
+   * f5_ln_modulate launches; anything else is F5_ERR_INVALID.  ln_tab_ld = depth*(3D + ff_inner) + 128
+   * (f5_dit_ln_tab_ld). */
   float* ln_stats;            /* fp32 [rows, D/64, 2]: per-row (sum, sum of squares) per 64 columns of the residual stream */
   float* ln_tab;              /* fp32 [4*n_times, ln_tab_ld]: c1/c2 operand rows per time, columns = per block [qkv 3D | ff1 F], then proj_out */
   void* ln_prep;              /* bf16 [2*depth+1, 4*n_times, D]: operand rows of the table GEMMs */
@@ -337,11 +328,12 @@ typedef struct f5_dit_buffers {
    * masked as attention keys, so rows < N equal the unpadded computation.  NULL = all `frames` rows are real. */
   const int32_t* valid_len;   /* int32 [rows/frames], every entry the same N <= frames, or NULL */
   /* FP8 mode: e4m3 [rows, D] — the AdaLN-modulated operand of the QKV / FF1 GEMMs (written by the producing GEMM's
-   * epilogue instead of a_bf16); requires the fused AdaLN buffers and blocks[i].qkv_w8 / ff1_w8.  NULL = bf16. */
+   * epilogue instead of a_bf16); requires the fused AdaLN buffers and all four blocks[i].*_w8.  NULL = bf16. */
   void* a_fp8;
   /* Block-scaled FP8 mode (ABI 1.101): per (row, 64-column unit) scales, unit-major — fp32 [D/64][rows] of a_fp8, fp32
    * [heads][rows] of the attention output (e4m3 in c_bf16), fp32 [ff_inner/64][rows] of the FF1 output (e4m3 in
-   * ff_bf16).  NULL = per-tensor FP8 (or bf16).  F5_FP8_LEVEL has no effect in this mode. */
+   * ff_bf16).  All three set selects the mode and requires a_fp8 and all four blocks[i].*_ws; all three NULL =
+   * per-tensor FP8 (or bf16). */
   float* a_fp8_scale;
   float* attn_scale;
   float* ff_scale;

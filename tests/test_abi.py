@@ -81,6 +81,17 @@ def test_product_package_never_imports_the_oracle():
                 assert not pat.search(src), f"{fn} imports the oracle"
 
 
+def test_library_reads_no_environment_variables():
+    """What the library computes depends on its arguments alone: no environment variable selects another code path
+    that the tests and the benchmark never run."""
+    csrc = os.path.join(ROOT, "f5_tts_mlx_b200", "csrc")
+    srcs = sorted(os.listdir(csrc))
+    assert any(fn.endswith(".cu") for fn in srcs)
+    for fn in srcs:
+        src = open(os.path.join(csrc, fn)).read()
+        assert not re.search(r"\bgetenv\b", src), f"csrc/{fn} calls getenv"
+
+
 def test_header_is_plain_c99_and_links_from_c(tmp_path):
     """include/f5_b200.h compiles as strict C99 and a C program links against libf5b200.so: the boundary has no
     C++ or torch types.  The consumer also checks that the C compiler's struct layout equals the library's."""

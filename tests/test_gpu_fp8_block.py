@@ -304,3 +304,47 @@ def test_block_mode_sample_through_from_pretrained():
     one, _ = f5.sample(cond[:1], text[:1], 250, steps=4, method="euler", cfg_strength=2.0, seed=1, frame_bucket=128)
     assert one.shape[1] == 250 and torch.isfinite(one).all()
     assert f5.last_plan.session.frames == 256 and f5.last_plan.session.a_fp8_scale is not None
+
+
+def test_dit_forward_rejects_a_partly_bound_mode():
+    """f5_dit_forward checks the mode its buffers and weights select instead of inferring one from whichever pointers
+    are set: a partly bound fused-AdaLN, FP8 or block-scaled set is F5_ERR_INVALID naming what is missing."""
+    import ctypes as C
+    from f5_tts_mlx_b200 import _lib
+    from f5_tts_mlx_b200.dit import DitBuffersC
+    from f5_tts_mlx_b200.weights import GATE_CONFIG, DitBlockWeightsC, DitWeightsC, random_dit_weights
+    cfg = GATE_CONFIG
+    W = random_dit_weights(cfg, seed=1234)
+    lib = _lib.load()
+
+    def forward(model, unbind=(), unbind_block=None):
+        s = model.session(1, 128, 1, False, 16, False)
+        b = DitBuffersC.from_buffer_copy(s.c)
+        for name in unbind:
+            setattr(b, name, None)
+        w = DitWeightsC.from_buffer_copy(model.packed.c_struct())
+        blks = (DitBlockWeightsC * cfg.depth)(*[DitBlockWeightsC.from_buffer_copy(w.blocks[i])
+                                                for i in range(cfg.depth)])
+        if unbind_block is not None:
+            i, names = unbind_block
+            for name in names:
+                setattr(blks[i], name, None)
+        w.blocks = blks
+        rc = lib.f5_dit_forward(C.byref(w), C.byref(b), 0, C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        return rc, lib.f5_last_error().decode()
+
+    bf16, tensor, block = _dit(cfg, W), _dit(cfg, W, fp8=True), _dit(cfg, W, fp8=True, fp8_scaling="block")
+    rc, msg = forward(bf16, unbind=("ln_prep",))
+    assert rc == -1 and "fused AdaLN needs ln_prep" in msg, msg
+    rc, msg = forward(tensor, unbind=("ln_stats", "ln_tab", "ln_prep"))
+    assert rc == -1 and "FP8 needs the fused AdaLN" in msg, msg
+    rc, msg = forward(tensor, unbind_block=(1, ("out_w8", "ff2_w8")))
+    assert rc == -1 and "FP8 needs out_w8, ff2_w8 of blocks[1]" in msg, msg
+    rc, msg = forward(block, unbind=("attn_scale",))
+    assert rc == -1 and "block-scaled FP8 needs attn_scale" in msg, msg
+    rc, msg = forward(block, unbind=("a_fp8",))
+    assert rc == -1 and "FP8 needs a_fp8" in msg, msg
+    rc, msg = forward(block, unbind=("a_fp8_scale", "attn_scale", "ff_scale"))
+    assert rc == -1 and "blocks[0] has per-channel weight scales" in msg, msg
+    rc, msg = forward(block, unbind_block=(0, ("ff1_ws",)))
+    assert rc == -1 and "block-scaled FP8 needs ff1_ws of blocks[0]" in msg, msg

@@ -55,7 +55,8 @@ def row_lens(nb, rpb):
 
 def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.0, rpb=0, nb=1, batched=False,
               row_len=False, gate=None, resid=None, out2=None, ln_scale=False, rope=False, ab8=False, pad_cols=0):
-    """One GEMM launch against its float64 reference.  out: 'bf16' | 'f32' | 'e4m3'; gate: None | 'shared' | 'utt';
+    """One GEMM launch against its float64 reference.  out: 'bf16' | 'f32' | 'e4m3'; gate: None | 'shared' (one [N]
+    vector for every utterance);
     resid: None | 'alias' (resid is out itself) | 'sep'; out2: None | 'bf16' | 'e4m3'."""
     from f5_tts_mlx_b200 import ops
     odt = {"bf16": torch.bfloat16, "f32": torch.float32, "e4m3": torch.uint8}[out]
@@ -87,13 +88,9 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
         kw.update(row_len=lens)
     g_out = Guarded(M, N, odt, DEV, pad_cols=pad_cols)
     if gate is not None:
-        if gate == "shared":
-            gt = pow2((N,), seed + 4)
-            gm = gt.double()[None]
-        else:
-            gbuf = pow2((nb, N + 4), seed + 4)
-            gt = gbuf[:, :N]
-            gm = gt.double()[bidx]
+        assert gate == "shared"
+        gt = pow2((N,), seed + 4)
+        gm = gt.double()[None]
         v, vb = v * gm, vb * gm.abs()
         kw.update(gate=gt)
     if resid is not None:
@@ -176,11 +173,11 @@ def _epi():
         for batched in (False, True):
             for rpb in (1, 127, 129, 937):
                 nb = 300 if rpb == 1 else 3
-                for gate in ("shared", "utt"):
+                for gate in ("shared", None):
                     if gate == "shared":   # the block's out-projection / FF2: fp32 stream updated in place
                         cases.append(dict(M=rpb * nb, N=100, K=200, tile=tile, w_static=1, rpb=rpb, nb=nb, batched=batched,
                                           row_len=True, gate=gate, resid="alias", out="f32"))
-                    else:
+                    else:                  # a separate residual without a gate, bf16 output
                         cases.append(dict(M=rpb * nb, N=136, K=200, tile=tile, w_static=0, rpb=rpb, nb=nb, batched=batched,
                                           row_len=True, gate=gate, resid="sep", out="bf16"))
     return cases

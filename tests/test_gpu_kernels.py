@@ -87,27 +87,29 @@ def test_gemm_qkv_rope_epilogue():
 _declare(out_dtype=torch.float32, resid=True)
 
 
-def test_gemm_gate_mask_residual_inplace():
+def test_gemm_shared_gate_mask_residual_inplace():
+    """The out-projection / FF2 form: x = resid + gate * (a W^T + bias) in place, with one [D] gate for every utterance
+    and the rows past each utterance's length masked."""
     for tile in TILES:
-        _gate_mask_residual_inplace(tile)
+        _shared_gate_mask_residual_inplace(tile)
 
 
-def _gate_mask_residual_inplace(tile):
+def _shared_gate_mask_residual_inplace(tile):
     from f5_tts_mlx_b200 import ops
     B, NF, D = 2, 937, 1024
     M = B * NF
     a = rnd(M, 2048).bfloat16(); w = rnd(D, 2048, scale=2048 ** -0.5).bfloat16(); bias = rnd(D)
-    gate = rnd(B, 6 * D); x0 = rnd(M, D)
+    gate = rnd(6 * D); x0 = rnd(M, D)
     g = Guarded(M, D, torch.float32, dev)
     g.view.copy_(x0)
     lens = torch.tensor([937, 700], dtype=torch.int32, device=dev)
-    ops.gemm(a, w, g.view, bias=bias, resid=g.view, gate=gate[:, 2 * D:3 * D], row_len=lens, rows_per_batch=NF,
+    ops.gemm(a, w, g.view, bias=bias, resid=g.view, gate=gate[2 * D:3 * D], row_len=lens, rows_per_batch=NF,
              num_batches=B, tile_n=tile)
     v, b = lin(a, w, bias)
     valid = (torch.arange(M, device=dev) % NF < lens.repeat_interleave(NF))[:, None].double()
-    gm = gate[:, 2 * D:3 * D].double().repeat_interleave(NF, 0)
+    gm = gate[2 * D:3 * D].double()             # one gate vector shared by all utterances, as in the DiT
     ref = x0.double() + gm * v * valid
-    b = gm.abs() * b * valid + 2 * U32 * ref.abs()           # gate product and residual add, each rounded
+    b = gm.abs() * b * valid + 2 * U32 * ref.abs()           # gate product and residual add (one FMA)
     assert_within(g.view, ref, out_bound(ref, b, torch.float32), gemm_tiles(tile), f"gate/mask/resid tile {tile}")
     g.check("gate/mask/resid guard")
 
@@ -203,12 +205,11 @@ def _producer_check(g, g2, st, x, bx, s, out2_dtype, loc, what):
 _declare(out_dtype=torch.float32, resid=True)
 
 
-@pytest.mark.parametrize("M,D,K,variant,tile", [(1874, 1024, 1024, 1, 0), (1874, 1024, 2048, 1, 0), (300, 512, 512, 1, 64),
-                                                (700, 1024, 1024, 2, 256), (40000, 1024, 2048, 0, 0)])
-def test_gemm_fused_ln_producer(M, D, K, variant, tile):
+@pytest.mark.parametrize("M,D,K,tile", [(1874, 1024, 1024, 0), (1874, 1024, 2048, 0), (300, 512, 512, 64),
+                                        (700, 1024, 1024, 128), (40000, 1024, 2048, 0)])
+def test_gemm_fused_ln_producer(M, D, K, tile):
     """out-proj / FF2 shape: x = resid + gate * (a W^T + bias) in fp32, plus the bf16 operand x * (1 + s) and the
-    per-row unit statistics (sum, sum of squares per 64 columns) of x.  `variant` selects nothing on sm_90 and a 256
-    request runs 128-wide tiles; both stay accepted values of the ABI."""
+    per-row unit statistics (sum, sum of squares per 64 columns) of x."""
     from f5_tts_mlx_b200 import ops
     a = rnd(M, K).bfloat16(); w = rnd(D, K, scale=K ** -0.5).bfloat16(); bias = rnd(D)
     gate = rnd(1, D); x0 = rnd(M, D) * 2 + 0.3; s = rnd(D, seed=5) * 0.3
@@ -216,11 +217,11 @@ def test_gemm_fused_ln_producer(M, D, K, variant, tile):
     g2 = Guarded(M, D, torch.bfloat16, dev)
     st = Guarded(M, D // 64 * 2, torch.float32, dev, lr=False)
     ops.gemm(a, w, g.view, bias=bias, resid=g.view, gate=gate[0], out2=g2.view, ln_scale=s,
-             ln_stats=st.view.view(M, D // 64, 2), variant=variant, tile_n=tile, w_static=True)
+             ln_stats=st.view.view(M, D // 64, 2), tile_n=tile, w_static=True)
     v, b = lin(a, w, bias)
     x = x0.double() + gate.double() * v
     bx = gate.double().abs() * b + U32 * x.abs()
-    _producer_check(g, g2, st, x, bx, s, torch.bfloat16, gemm_tiles(min(tile, 128) or 64), f"ln producer tile {tile}")
+    _producer_check(g, g2, st, x, bx, s, torch.bfloat16, gemm_tiles(tile or 64), f"ln producer tile {tile}")
 
 
 def _ln_tab(scale, shift, w):
@@ -472,9 +473,9 @@ def test_dwconv7_ln_and_grn():
 _declare(fp8=True)
 
 
-@pytest.mark.parametrize("M,N,K,variant,tile,act", [(1874, 3072, 1024, 0, 0, 0), (1874, 2048, 1024, 0, 0, 1), (300, 256, 128, 1, 0, 0),
-                                                     (257, 512, 256, 1, 64, 0), (700, 1024, 1024, 2, 256, 0), (40000, 2048, 1024, 0, 0, 1)])
-def test_gemm_fp8_operands(M, N, K, variant, tile, act):
+@pytest.mark.parametrize("M,N,K,tile,act", [(1874, 3072, 1024, 0, 0), (1874, 2048, 1024, 0, 1), (300, 256, 128, 0, 0),
+                                             (257, 512, 256, 64, 0), (700, 1024, 1024, 128, 0), (40000, 2048, 1024, 0, 1)])
+def test_gemm_fp8_operands(M, N, K, tile, act):
     """f5_gemm_args.ab_fp8: A and W as e4m3 bytes, accumulator x acc_scale + bias (+ GELU), bf16 out — against the
     float64 product of the SAME e4m3 values.  The explicit tile widths of FP8 GELU run in the chain tests below."""
     from f5_tts_mlx_b200 import ops
@@ -482,10 +483,10 @@ def test_gemm_fp8_operands(M, N, K, variant, tile, act):
     sc = float(wf.abs().max()) / 448.0
     w8 = e4m3(wf / sc)
     g = Guarded(M, N, torch.bfloat16, dev)
-    ops.gemm(a8, w8, g.view, bias=bias, act=act, ab_fp8=True, acc_scale=sc, variant=variant, tile_n=tile)
+    ops.gemm(a8, w8, g.view, bias=bias, act=act, ab_fp8=True, acc_scale=sc, tile_n=tile)
     v, b = lin(a8, w8, bias, sc, fp8=True)
     ref = act_ref(v, act)
-    assert_within(g.view, ref, out_bound(ref, act_bound(v, b, act), torch.bfloat16), gemm_tiles(min(tile, 128) or 64),
+    assert_within(g.view, ref, out_bound(ref, act_bound(v, b, act), torch.bfloat16), gemm_tiles(tile or 64),
                   f"fp8 act {act} tile {tile}")
     g.check("fp8 guard")
 
