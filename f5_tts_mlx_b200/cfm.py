@@ -332,10 +332,13 @@ class F5TTS:
         return out, trajectory
 
     @classmethod
-    def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None):
-        """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8)."""
+    def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None,
+                        fp8_attention=False):
+        """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8);
+        fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well."""
         from .pretrained import from_pretrained
-        return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8)
+        return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8,
+                               fp8_attention=fp8_attention)
 
 
 CFM = F5TTS

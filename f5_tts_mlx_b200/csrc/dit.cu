@@ -19,6 +19,10 @@ extern "C" int f5_attention_fwd_e4m3(const void*, int64_t, void*, int64_t, int32
                                      int32_t, const int32_t*, void*);
 extern "C" int f5_attention_fwd_e4m3_scaled(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
                                             int32_t, const int32_t*, float*, void*);
+extern "C" int f5_qkv_quant_e4m3(const void*, int64_t, void*, int64_t, void*, int64_t, float*, int32_t, int32_t,
+                                 int32_t, void*);
+extern "C" int f5_attention_fwd_fp8(const void*, int64_t, const void*, int64_t, const float*, void*, int64_t, int32_t,
+                                    int32_t, int32_t, int32_t, const int32_t*, float*, void*);
 
 namespace f5 {
 
@@ -41,6 +45,7 @@ struct DitMode {
   bool fused;   // AdaLN LayerNorm folded into the GEMM epilogues (ln_stats / ln_tab / ln_prep)
   bool fp8;     // the four block GEMMs on e4m3 operands (a_fp8)
   bool blk8;    // ... with block scales (a_fp8_scale / attn_scale / ff_scale)
+  bool attn8;   // ... and the attention on e4m3 Q, K, V (qk_fp8 / vt_fp8 / qkv_scale)
 };
 
 struct NamedPtr { const char* name; const void* p; };
@@ -72,6 +77,12 @@ static int check_mode(const f5_dit_weights* w, const f5_dit_buffers* b, DitMode&
     if (int e = need_all("block-scaled FP8", -1, {{"a_fp8_scale", b->a_fp8_scale}, {"attn_scale", b->attn_scale},
                                                   {"ff_scale", b->ff_scale}}))
       return e;
+  m.attn8 = b->qk_fp8 || b->vt_fp8 || b->qkv_scale;
+  if (m.attn8) {
+    if (int e = need_all("FP8 attention", -1, {{"qk_fp8", b->qk_fp8}, {"vt_fp8", b->vt_fp8}, {"qkv_scale", b->qkv_scale}}))
+      return e;
+    F5_REQUIRE(m.blk8, "dit: FP8 attention needs the block-scaled FP8 mode (a_fp8_scale, attn_scale and ff_scale)");
+  }
   for (int l = 0; m.fp8 && l < w->depth; ++l) {
     const f5_dit_block_weights& bw = w->blocks[l];
     if (int e = need_all("FP8", l, {{"qkv_w8", bw.qkv_w8}, {"ff1_w8", bw.ff1_w8}, {"out_w8", bw.out_w8},
@@ -261,7 +272,16 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       if (prefetch && blk8) { g.prefetch = bw.out_w8; g.prefetch_bytes = (int64_t)D * D; }   // the e4m3 weights it reads
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
-    if (blk8) {
+    if (mode.attn8) {
+      const int64_t vt_ld = (int64_t)cdiv(N, 128) * 128;
+      const int32_t* kv_len = b->seq_len ? b->seq_len : b->valid_len;
+      if (int e = f5_qkv_quant_e4m3(b->qkv_bf16, 3 * D, b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, BU, N,
+                                    w->heads, st))
+        return e;
+      if (int e = f5_attention_fwd_fp8(b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, b->c_bf16, D, BU, N, w->heads,
+                                       64, kv_len, b->attn_scale, st))
+        return e;
+    } else if (blk8) {
       if (int e = f5_attention_fwd_e4m3_scaled(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
                                                b->seq_len ? b->seq_len : b->valid_len, b->attn_scale, st))
         return e;

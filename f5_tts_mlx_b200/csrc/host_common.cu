@@ -65,7 +65,8 @@ static PFN_encodeTiled get_encode() {
 }
 
 static int make_tmap_any(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                         const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapDataType dt);
+                         const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapDataType dt,
+                         CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B);
 int make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                    const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap_any(map, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
@@ -74,8 +75,14 @@ int make_tmap_u8(CUtensorMap* map, const void* base, int rank, const uint64_t* d
                  const uint64_t* strides_bytes, const uint32_t* box) {
   return make_tmap_any(map, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_DATA_TYPE_UINT8);
 }
+int make_tmap_u8_sw64(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                      const uint64_t* strides_bytes, const uint32_t* box) {
+  return make_tmap_any(map, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_DATA_TYPE_UINT8,
+                       CU_TENSOR_MAP_SWIZZLE_64B);
+}
 static int make_tmap_any(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
-                         const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapDataType dt) {
+                         const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapDataType dt,
+                         CUtensorMapSwizzle swz) {
   PFN_encodeTiled enc = get_encode();
   if (!enc) return set_error(F5_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint64_t gdim[5];
@@ -96,7 +103,7 @@ static int make_tmap_any(CUtensorMap* map, const void* base, int rank, const uin
                        (unsigned long long)gstr[i]);
   CUresult r = enc(map, dt, (cuuint32_t)rank, const_cast<void*>(base),
                    gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return set_error(F5_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
@@ -186,6 +193,6 @@ int f5_struct_sizes(int32_t* out, int32_t n) {
   return 10;
 }
 const char* f5_last_error(void) { return f5::g_err; }
-int f5_abi_version(void) { return 2000; }
+int f5_abi_version(void) { return 2001; }
 int f5_device_check(void) { return f5::device_check(); }
 }

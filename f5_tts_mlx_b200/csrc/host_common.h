@@ -36,6 +36,9 @@ int make_tmap_bf16(CUtensorMap* map, const void* base, int rank, const uint64_t*
 // the same for 1-byte elements (e4m3 operands of the FP8 mode): 128-byte swizzle, box[0] = 128 elements
 int make_tmap_u8(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                  const uint64_t* strides_bytes, const uint32_t* box);
+// 1-byte elements with the 64-byte swizzle: rows of 64 e4m3 (box[0] = 64), the FP8 attention's Q and K tiles
+int make_tmap_u8_sw64(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
+                      const uint64_t* strides_bytes, const uint32_t* box);
 // Tensor map of an OUTPUT matrix for the GEMM epilogue's TMA stores: elem_bytes 4 (fp32, 32-column boxes = 128 B rows,
 // 128-byte swizzle), 2 (bf16, 32-column boxes = 64 B rows, 64-byte swizzle) or 1 (e4m3, 32 B rows, 32-byte swizzle);
 // dims (cols, rows per utterance, utterances).

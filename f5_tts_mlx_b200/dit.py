@@ -29,6 +29,7 @@ class DitBuffersC(C.Structure):
         ("ln_stats", C.c_void_p), ("ln_tab", C.c_void_p), ("ln_prep", C.c_void_p),
         ("valid_len", C.c_void_p), ("a_fp8", C.c_void_p),
         ("a_fp8_scale", C.c_void_p), ("attn_scale", C.c_void_p), ("ff_scale", C.c_void_p),
+        ("qk_fp8", C.c_void_p), ("vt_fp8", C.c_void_p), ("qkv_scale", C.c_void_p),
     ]
 
 
@@ -48,7 +49,7 @@ class DitSession:
 
     def __init__(self, cfg: DiTConfig, ct_ld: int, batch: int, frames: int, n_times: int, use_cfg: bool,
                  text_cols: int, device: torch.device, masked: bool, fused_adaln: bool = True, fp8: bool = False,
-                 fp8_block: bool = False):
+                 fp8_block: bool = False, fp8_attention: bool = False):
         self.cfg, self.batch, self.frames, self.n_times, self.use_cfg = cfg, batch, frames, n_times, use_cfg
         self.device = device
         D, F, Ct = cfg.dim, cfg.ff_inner, cfg.text_dim
@@ -96,6 +97,11 @@ class DitSession:
         self.a_fp8_scale = z(D // 64, R) if blk else None
         self.attn_scale = z(cfg.heads, R) if blk else None
         self.ff_scale = z(F // 64, R) if blk else None
+        # FP8 attention: e4m3 Q | K, e4m3 V^T with keys padded to a multiple of 128 (zeros), scales [3 heads][rows]
+        att8 = blk and fp8_attention
+        self.qk_fp8 = z(R, 2 * D, dt=torch.uint8) if att8 else None
+        self.vt_fp8 = z(BU, D, (frames + 127) // 128 * 128, dt=torch.uint8) if att8 else None
+        self.qkv_scale = z(3 * cfg.heads, R) if att8 else None
         c = DitBuffersC()
         c.batch, c.frames, c.cfg, c.n_times = batch, frames, int(use_cfg), n_times
         c.text_len_max, c.drop_flags = self.text.shape[1], 0
@@ -150,7 +156,7 @@ class DiT:
     def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.0, ff_mult=4, mel_dim=100,
                  text_num_embeds=256, text_dim=None, text_mask_padding=True, conv_layers=0,
                  device: str | torch.device = "cuda", fused_adaln: bool = True, fp8: bool = False,
-                 fp8_scaling: str = "tensor"):
+                 fp8_scaling: str = "tensor", fp8_attention: bool = False):
         if text_dim is None:
             text_dim = mel_dim
         if dim_head != 64 or dim != heads * dim_head:
@@ -184,6 +190,11 @@ class DiT:
             raise ValueError(f"fp8_scaling must be one of {FP8_SCALINGS}, not {fp8_scaling!r}")
         self.fp8_scaling = fp8_scaling
         self.fp8_block = self.fp8 and fp8_scaling == "block"
+        # fp8_attention: the attention's Q·K^T and P·V also on e4m3, with power-of-two scales per (row, head) of Q and
+        # per (utterance, head, 128-key tile) of K and V (DESIGN.md sections 5 and 8); lossy like the rest of the mode
+        if fp8_attention and not self.fp8_block:
+            raise ValueError('fp8_attention=True needs fp8=True and fp8_scaling="block" (its scales are per (row, head))')
+        self.fp8_attention = bool(fp8_attention)
         self.device = torch.device(device)
         self.packed: Optional[PackedDiT] = None
         self._sessions: Dict[tuple, DitSession] = {}
@@ -212,13 +223,14 @@ class DiT:
     # -- sessions --
     def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int,
                 masked: bool, bucketed: bool = False) -> DitSession:
-        key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8, self.fp8_block)
+        key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8, self.fp8_block,
+               self.fp8_attention)
         s = self._sessions.pop(key, None)
         if s is None:
             while len(self._sessions) >= self.session_cache_size:
                 self._sessions.pop(next(iter(self._sessions)))
             s = DitSession(self.config, self._require_weights().ct_ld, batch, frames, n_times, use_cfg,
-                           text_cols, self.device, masked, self.fused_adaln, self.fp8, self.fp8_block)
+                           text_cols, self.device, masked, self.fused_adaln, self.fp8, self.fp8_block, self.fp8_attention)
             if bucketed:
                 s.use_bucketing()
         self._sessions[key] = s          # LRU order: most recently used last

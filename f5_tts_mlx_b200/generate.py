@@ -95,6 +95,7 @@ def generate(
     batch_sentences: bool = False,
     frame_bucket: int = 128,
     fp8: Optional[str] = None,
+    fp8_attention: bool = False,
 ):
     """generate.py:113-244.  Extensions: `f5tts` reuses a loaded model; `batch_sentences=True` runs all
     sentences as ONE ragged `sample()` batch instead of the reference's serial loop
@@ -102,9 +103,13 @@ def generate(
     statistics and the ODE on padded frames see the batch-maximum length); `frame_bucket` (default 128 frames) lets
     the sentences of the serial loop share one set of buffers and ONE captured CUDA graph per length bucket instead of
     re-capturing for every distinct length (0 = the exact shapes); results are unchanged (F5TTS.sample).  `fp8`: None
-    (bf16), "tensor" or "block" — the lossy FP8 mode of the DiT and its scaling (DESIGN.md section 8)."""
+    (bf16), "tensor" or "block" — the lossy FP8 mode of the DiT and its scaling (DESIGN.md section 8);
+    `fp8_attention` (with fp8="block"): the attention on e4m3 Q, K and V as well."""
+    if fp8_attention and fp8 != "block":
+        raise ValueError('fp8_attention needs fp8="block"')
     if f5tts is None:
-        f5tts = F5TTS.from_pretrained(model_name, quantization_bits=quantization_bits, fp8=fp8)
+        f5tts = F5TTS.from_pretrained(model_name, quantization_bits=quantization_bits, fp8=fp8,
+                                      fp8_attention=fp8_attention)
     dev = f5tts.transformer.device
     if f5tts._vocoder is None:
         raise ValueError("generate() needs a model with a vocoder (F5TTS(..., vocoder=Vocos(...).decode)); "
@@ -191,7 +196,11 @@ def main(argv=None) -> None:
     p.add_argument("--q", type=int, default=None, choices=[4, 8])
     p.add_argument("--fp8", type=str, default=None, choices=["tensor", "block"],
                    help="run the DiT's GEMMs on e4m3 operands (lossy) with per-tensor or block (per-channel / per-64) scales")
+    p.add_argument("--fp8-attention", action="store_true",
+                   help="with --fp8 block: run the attention's Q·K^T and P·V on e4m3 too (lossy)")
     a = p.parse_args(argv)
+    if a.fp8_attention and a.fp8 != "block":
+        p.error("--fp8-attention needs --fp8 block")
     if a.text is None:
         import sys
         if not sys.stdin.isatty():
@@ -201,7 +210,7 @@ def main(argv=None) -> None:
     generate(generation_text=a.text, duration=a.duration, estimate_duration=a.estimate_duration, model_name=a.model,
              ref_audio_path=a.ref_audio, ref_audio_text=a.ref_text, steps=a.steps, method=a.method, cfg_strength=a.cfg,
              sway_sampling_coef=a.sway_coef, speed=a.speed, seed=a.seed, quantization_bits=a.q, output_path=a.output,
-             fp8=a.fp8)
+             fp8=a.fp8, fp8_attention=a.fp8_attention)
 
 
 if __name__ == "__main__":

@@ -95,17 +95,17 @@ def convert_vocos_upstream(w: Weights) -> Weights:
 
 def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits: Optional[int] = None,
                     device: str | torch.device = "cuda", vocab_path: Optional[str] = None, vocoder=None,
-                    fp8: Optional[str] = None):
+                    fp8: Optional[str] = None, fp8_attention: bool = False):
     """`vocoder`: None = resolve and REQUIRE one (reference behaviour), False = none (sample() returns mels),
     or a callable mel -> waveform.  `fp8`: None = bf16, "tensor" or "block" = the DiT's FP8 mode with that weight /
     activation scaling (DESIGN.md section 8); the weights (dequantised first for quantization_bits) are quantised to
-    e4m3 at pack time."""
+    e4m3 at pack time.  `fp8_attention` (needs fp8="block"): the attention on e4m3 Q, K and V as well."""
     import os
     if quantization_bits is not None and quantization_bits not in (4, 8):
         raise ValueError(f"quantization_bits must be 4 or 8 (generate.py --q), got {quantization_bits}")
     if fp8 is not None and fp8 not in FP8_SCALINGS:
         raise ValueError(f"fp8 must be None or one of {FP8_SCALINGS}, got {fp8!r}")
-    fp8_kw = dict(fp8=fp8 is not None, fp8_scaling=fp8 or "tensor")
+    fp8_kw = dict(fp8=fp8 is not None, fp8_scaling=fp8 or "tensor", fp8_attention=fp8_attention)
     if hf_model_name_or_path == "random":
         vp = vocab_path or os.environ.get("F5_VOCAB_PATH")
         if vp is not None:

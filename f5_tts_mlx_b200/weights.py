@@ -321,6 +321,15 @@ def quantize_e4m3_blocks(x: torch.Tensor, block: int = 64):
     return q.view(torch.uint8).reshape(r, c), s
 
 
+def fp8_vt_key_order() -> torch.Tensor:
+    """Key order of the FP8 attention's V^T (f5_qkv_quant_e4m3): position p of every 32-key group holds key
+    order[p].  It makes the softmax's S accumulator fragment (keys {2l, 2l+1, 2l+8, 2l+9} and 16 + those, l = lane % 4)
+    the e4m3 register A fragment of the P·V wgmma (k = 4l .. 4l+3 and 16 + those): position 16 h + 4 l + i holds key
+    16 h + (2l, 2l+1, 2l+8, 2l+9)[i] (csrc/attention_fp8_sm90.cuh fp8_vt_key)."""
+    p = torch.arange(32)
+    return (p & 16) + 2 * ((p >> 2) & 3) + 8 * ((p >> 1) & 1) + (p & 1)
+
+
 class DitWeightsC(C.Structure):
     _fields_ = [
         ("dim", C.c_int32), ("depth", C.c_int32), ("heads", C.c_int32), ("ff_inner", C.c_int32),

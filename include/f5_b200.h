@@ -160,6 +160,22 @@ int f5_attention_fwd_e4m3(const void* qkv, int64_t ld_qkv, void* out, int64_t ld
 int f5_attention_fwd_e4m3_scaled(const void* qkv, int64_t ld_qkv, void* out, int64_t ld_out, int32_t batch,
                                  int32_t frames, int32_t heads, int32_t head_dim, const int32_t* kv_len,
                                  float* scale_out, void* stream);
+/* FP8 attention of the block-scaled FP8 mode (ABI 2.001): e4m3 Q·K^T and P·V with power-of-two scales, one per
+ * (row, head) of Q and one per (utterance, head, 128-key tile) of K and of V.
+ * f5_qkv_quant_e4m3    : qkv bf16 [batch*frames, ld_qkv] as above -> qk8 e4m3 [batch*frames, ld_qk8] = [q | k]
+ *                        (ld_qk8 bytes, multiple of 16), vt8 e4m3 [batch][heads*64][vt_ld] = V transposed with keys
+ *                        contiguous, in the order of weights.fp8_vt_key_order() within every 32 keys, zero for keys
+ *                        in [frames, roundup(frames, 128)) (vt_ld bytes, multiple of 16, >= roundup(frames, 128)), and
+ *                        qkv_scale fp32 [3*heads][batch*frames]: q head h -> unit h, k head h -> heads + h, v head h ->
+ *                        2*heads + h (the scale rule of f5_gemm_args.a_scale, applied to the bf16 values; every k and v row holds
+ *                        the scale of its 128-key tile).
+ * f5_attention_fwd_fp8 : attention on those operands; out / scale_out as f5_attention_fwd_e4m3_scaled.
+ * Pointers 16-byte aligned. */
+int f5_qkv_quant_e4m3(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8, int64_t vt_ld,
+                      float* qkv_scale, int32_t batch, int32_t frames, int32_t heads, void* stream);
+int f5_attention_fwd_fp8(const void* qk8, int64_t ld_qk8, const void* vt8, int64_t vt_ld, const float* qkv_scale,
+                         void* out, int64_t ld_out, int32_t batch, int32_t frames, int32_t heads, int32_t head_dim,
+                         const int32_t* kv_len, float* scale_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
  * HBM-bound pieces.
@@ -337,6 +353,12 @@ typedef struct f5_dit_buffers {
   float* a_fp8_scale;
   float* attn_scale;
   float* ff_scale;
+  /* FP8 attention (ABI 2.001, see f5_attention_fwd_fp8): e4m3 [rows, 2D] Q | K, e4m3 [rows/frames][D][roundup(frames,
+   * 128)] V^T and fp32 [3*heads][rows] scales.  All three set selects it inside the block-scaled FP8 mode (which it
+   * requires); all three NULL keeps the bf16 attention with a block-scaled e4m3 output. */
+  void* qk_fp8;
+  void* vt_fp8;
+  float* qkv_scale;
 } f5_dit_buffers;
 
 /* step-invariant work, once per sample(): text embedding (dit.py:196-229), hoisted conditioning
