@@ -43,19 +43,26 @@ def q_tiles(x: torch.Tensor):
     return E._quant(x.float(), s).double(), s.double()
 
 
-def attention_fp8(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask) -> torch.Tensor:
-    """q, k, v: [b, h, n, 64] bf16 values (q already scaled by 1/8); mask [b, n] bool or None -> O [b, h, n, 64]."""
+def attention_fp8(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask, heads_per_chunk: int = 4) -> torch.Tensor:
+    """q, k, v: [b, h, n, 64] bf16 values (q already scaled by 1/8); mask [b, n] bool or None -> O [b, h, n, 64].
+    The float64 scores are formed `heads_per_chunk` heads at a time (a [b, h, n, n] tensor is 8 GB at n = 5625), on
+    the GPU when there is one (the result returns to q's device)."""
     qc, sq = q_heads(q)
     kc, sk = q_tiles(k)
     vc, sv = q_tiles(v)
-    b, _, n, _ = q.shape
-    valid = mask.bool() if mask is not None else torch.ones(b, n, dtype=torch.bool)
-    s = (qc @ kc.transpose(-1, -2)) * sq * sk.transpose(-1, -2)
-    s = s.masked_fill(~valid[:, None, None, :], float("-inf"))
-    p = torch.exp(s - s.amax(-1, keepdim=True))
-    pt = E._quant(p * 256.0, torch.ones(())).double()
-    o = pt @ (vc * sv / 256.0)          # sv is constant over each tile: sum_t (sv_t / 2^8) P~_t V-codes_t
-    return (o / p.sum(-1, keepdim=True)).float()
+    b, h, n, _ = q.shape
+    dev = "cuda" if torch.cuda.is_available() else "cpu"
+    valid = (mask.bool() if mask is not None else torch.ones(b, n, dtype=torch.bool)).to(dev)
+    out = torch.empty(b, h, n, q.shape[-1])
+    for h0 in range(0, h, heads_per_chunk):
+        c = lambda t: t[:, h0:h0 + heads_per_chunk].to(dev)
+        s = (c(qc) @ c(kc).transpose(-1, -2)) * c(sq) * c(sk).transpose(-1, -2)
+        s = s.masked_fill(~valid[:, None, None, :], float("-inf"))
+        p = torch.exp(s - s.amax(-1, keepdim=True))
+        pt = E._quant(p * 256.0, torch.ones((), device=dev)).double()
+        o = pt @ (c(vc) * c(sv) / 256.0)    # sv is constant over each tile: sum_t (sv_t / 2^8) P~_t V-codes_t
+        out[:, h0:h0 + heads_per_chunk] = (o / p.sum(-1, keepdim=True)).float().cpu()
+    return out.to(q.device)
 
 
 def attention8a(x, mask, rope, W, pfx, heads, scale_msa, shift_msa):

@@ -45,18 +45,19 @@ def weights(name):
 _M = {}
 
 
-def model(name, depth=None, fused=True, fp8=None):
+def model(name, depth=None, fused=True, fp8=None, fp8_attention=False):
     """DiT `name` truncated to its first `depth` blocks (the packer reads blocks < depth of the full weights)."""
     from f5_tts_mlx_b200 import DiT
     cfg, W = weights(name)
     depth = cfg.depth if depth is None else depth
-    key = (name, depth, fused, fp8)
+    key = (name, depth, fused, fp8, fp8_attention)
     if key not in _M:
         c = dataclasses.replace(cfg, depth=depth)
         if fp8:
+            kw = dict(fp8_attention=True) if fp8_attention else {}
             _M[key] = DiT(dim=c.dim, depth=c.depth, heads=c.heads, ff_mult=c.ff_mult, mel_dim=c.mel_dim,
                           text_num_embeds=c.text_num_embeds, text_dim=c.text_dim, conv_layers=c.conv_layers,
-                          device=dev, fp8=True, fp8_scaling=fp8).load_weights(W)
+                          device=dev, fp8=True, fp8_scaling=fp8, **kw).load_weights(W)
         else:
             _M[key] = make_dit(c, W, fused_adaln=fused)
     return _M[key]
@@ -79,8 +80,10 @@ def oracle_mod_table(W, cfg, tvals, prec):
     return torch.cat(rows, -1)
 
 
-def oracle_stages(W, cfg, x, cond, text, t, drops, mask, prec, block8=False):
-    """One CFG branch of dit_forward, stage by stage: text_x, hoist, h, xs (after each block), v."""
+def oracle_stages(W, cfg, x, cond, text, t, drops, mask, prec, block8=False, attn8=False):
+    """One CFG branch of dit_forward, stage by stage: text_x, hoist, h, xs (after each block), v.  block8: the blocks
+    of the block-scaled FP8 mode (fp8_block_emul); attn8: those of its FP8 attention mode (fp8_attn_emul)."""
+    import fp8_attn_emul as A
     import fp8_block_emul as E
     B, N = x.shape[:2]
     temb = O.timestep_embedding(t.reshape(1).repeat(B).float(), W)
@@ -93,7 +96,12 @@ def oracle_stages(W, cfg, x, cond, text, t, drops, mask, prec, block8=False):
     rope = O.rotary_freqs(N, cfg.dim_head)
     xs = []
     for i in range(cfg.depth):
-        xx = E.dit_block8(xx, temb, mask, rope, W, i, cfg) if block8 else O.dit_block(xx, temb, mask, rope, W, i, cfg, prec)
+        if attn8:
+            xx = A.dit_block8a(xx, temb, mask, rope, W, i, cfg)
+        elif block8:
+            xx = E.dit_block8(xx, temb, mask, rope, W, i, cfg)
+        else:
+            xx = O.dit_block(xx, temb, mask, rope, W, i, cfg, prec)
         xs.append(xx)
     emb = O.linear(F.silu(temb), W["transformer.norm_out.linear.weight"], W["transformer.norm_out.linear.bias"], prec)
     scale, shift = emb.chunk(2, dim=1)
@@ -226,6 +234,42 @@ def test_fp8_forward_v_per_row(mode):
     report(f"fp8 {mode} v", assert_rows(got, ref, emu, what=f"fp8 {mode}: v"))
 
 
+# (model, depth, B, N, lens (ragged seq_len), bucket frames, block marks where x is checked)
+FP8A_CASES = [("gate", 4, 3, 150, [150, 131, 90], None, [1, 2, 3, 4]),
+              ("gate", 4, 3, 150, [150, 120, 97], 256, [1, 4]),
+              ("base", 2, 1, 5625, None, None, [1, 2])]
+
+
+@pytest.mark.parametrize("case", FP8A_CASES, ids=lambda c: f"{c[0]}-d{c[1]}-B{c[2]}-N{c[3]}{f'-bucket{c[5]}' if c[5] else ''}")
+def test_fp8_attention_stages_per_row(case):
+    """DiT(fp8=True, fp8_scaling="block", fp8_attention=True) with CFG: the residual stream x after each marked block
+    (depth-truncated models) and v, per row, against fp8_attn_emul's blocks.  The base model at N = 5625 (60 s) runs
+    the FP8 attention over 44 key tiles."""
+    name, depth, B, N, lens, NB, marks = case
+    cfg, W = weights(name)
+    ocfg = dataclasses.replace(ocfg_of(cfg), depth=depth)
+    NB = NB or N
+    x, cond, text = inputs(B, N, min(max(N // 3, 5) + 3, 512), seed=N * 10 + B)
+    if NB != N:
+        text = F.pad(text, (0, -(-text.shape[1] // 32) * 32 - text.shape[1]), value=-1)
+    tvals = eval_times("euler")
+    seq_len = torch.tensor(lens, dtype=torch.int32) if lens is not None else None
+    mask = (torch.arange(N)[None] < seq_len[:, None]) if lens is not None else None
+    brs = branches(True, 0)
+    ref = [oracle_stages(W, ocfg, x, cond, text, tvals[1], d, mask, O.FP32) for d in brs]
+    emu = [oracle_stages(W, ocfg, x, cond, text, tvals[1], d, mask, O.Precision(True, True), attn8=True) for d in brs]
+    view = lambda buf: buf.view(2, B, NB, -1)[:, :, :N].cpu()
+    tag = f"fp8 attention {name} B{B} N{N}{f' bucket{NB}' if NB != N else ''}"
+    for L in marks:
+        s = run_session(model(name, L, fp8="block", fp8_attention=True), x, cond, text, tvals, 1, seq_len, True, 0, NB)
+        report(f"{tag} x after block {L}",
+               assert_rows(view(s.x), torch.stack([r["xs"][L - 1] for r in ref]),
+                           torch.stack([r["xs"][L - 1] for r in emu]), what=f"{tag}: x after block {L}"))
+    assert marks[-1] == depth
+    report(f"{tag} v", assert_rows(view(s.v), torch.stack([r["v"] for r in ref]), torch.stack([r["v"] for r in emu]),
+                                   what=f"{tag}: v"))
+
+
 # ---------------------------------------------------------------- b. sample()
 def sample_inputs(B, N, seed):
     g = torch.Generator().manual_seed(seed)
@@ -258,6 +302,29 @@ def test_sample_out_and_last_state_per_row(method, steps, cfg_strength, B, bucke
     f5.use_cuda_graph = graph
     out, traj = f5.sample(cond.to(dev), text, dur, frame_bucket=bucket, **kw)
     tag = f"sample {method} cfg{cfg_strength:g} B{B} {'bucket' if bucket else 'exact'} {'graph' if graph else 'eager'}"
+    report(f"{tag} out", assert_rows(out.cpu()[None], ref[None], emu[None], what=f"{tag}: out"))
+    report(f"{tag} last state", assert_rows(traj[-1].cpu()[None], rtraj[-1][None], etraj[-1][None],
+                                            what=f"{tag}: trajectory[-1]"))
+
+
+@pytest.mark.parametrize("method,steps,bucket", [("euler", 4, 0), ("rk4", 3, 128)])
+def test_fp8_attention_sample_out_and_last_state_per_row(method, steps, bucket, monkeypatch):
+    """sample() in the FP8 attention mode, ragged batch of 3 with CFG, against the oracle's sample() whose DiT calls
+    are fp8_attn_emul.dit_forward_block8a."""
+    import fp8_attn_emul as A
+    from f5_tts_mlx_b200 import F5TTS
+    cfg, W = weights("gate")
+    B, N = 3, 150
+    cond, text, dur, y0 = sample_inputs(B, N, seed=steps * 10 + B + 1)
+    kw = dict(steps=steps, method=method, cfg_strength=2.0, sway_sampling_coef=-1.0, y0=y0)
+    ref, rtraj = O.sample(cond, text, dur, W, ocfg_of(cfg), **kw)
+    with monkeypatch.context() as mp:
+        mp.setattr(O, "dit_forward", lambda x, c, t, time, da, dt, mask, W, cfg, prec=None:
+                   A.dit_forward_block8a(x, c, t, time, da, dt, mask, W, cfg))
+        emu, etraj = O.sample(cond, text, dur, W, ocfg_of(cfg), **kw)
+    f5 = F5TTS(model("gate", fp8="block", fp8_attention=True))
+    out, traj = f5.sample(cond.to(dev), text, dur, frame_bucket=bucket, **kw)
+    tag = f"sample fp8 attention {method} B{B} {'bucket' if bucket else 'exact'}"
     report(f"{tag} out", assert_rows(out.cpu()[None], ref[None], emu[None], what=f"{tag}: out"))
     report(f"{tag} last state", assert_rows(traj[-1].cpu()[None], rtraj[-1][None], etraj[-1][None],
                                             what=f"{tag}: trajectory[-1]"))

@@ -315,12 +315,17 @@ INSTANTIATIONS = _declared()
 
 
 # ---------------------------------------------------------------- attention
-def _attn_call(qkv, out, B, N, H, kv_len, fp8=False):
+def _attn_call(qkv, out, B, N, H, kv_len, fp8=False, scale_out=None):
+    """f5_attention_fwd, f5_attention_fwd_e4m3 (fp8), or f5_attention_fwd_e4m3_scaled (scale_out [H, B N] given)."""
     from f5_tts_mlx_b200 import _lib
     lib = _lib.load()
-    fn = lib.f5_attention_fwd_e4m3 if fp8 else lib.f5_attention_fwd
-    _lib.check(fn(qkv.data_ptr(), qkv.stride(0), out.data_ptr(), out.stride(0), B, N, H, 64,
-                  kv_len.data_ptr() if kv_len is not None else None, torch.cuda.current_stream().cuda_stream))
+    args = (qkv.data_ptr(), qkv.stride(0), out.data_ptr(), out.stride(0), B, N, H, 64,
+            kv_len.data_ptr() if kv_len is not None else None)
+    stream = torch.cuda.current_stream().cuda_stream
+    if scale_out is not None:
+        _lib.check(lib.f5_attention_fwd_e4m3_scaled(*args, scale_out.data_ptr(), stream))
+    else:
+        _lib.check((lib.f5_attention_fwd_e4m3 if fp8 else lib.f5_attention_fwd)(*args, stream))
     torch.cuda.synchronize()
 
 
