@@ -102,6 +102,8 @@ SYMBOLS: dict[str, tuple] = {
                                                C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_qkv_quant_e4m3": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "f5_qkv_quant_e4m3_masked": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "f5_attention_fwd_fp8": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_ln_modulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,

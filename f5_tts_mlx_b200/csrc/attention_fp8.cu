@@ -4,8 +4,9 @@
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-extern "C" int f5_qkv_quant_e4m3(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8, int64_t vt_ld,
-                                 float* qkv_scale, int32_t batch, int32_t frames, int32_t heads, void* stream_) {
+extern "C" int f5_qkv_quant_e4m3_masked(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8,
+                                        int64_t vt_ld, float* qkv_scale, int32_t batch, int32_t frames, int32_t heads,
+                                        const int32_t* kv_len, void* stream_) {
   using namespace f5;
   if (int e = device_check()) return e;
   ProfScope ps(PROF_OTHER, 0.0, (double)batch * frames * heads * 64.0 * (2.0 * 3 + 3) + 12.0 * batch * frames * heads);
@@ -25,11 +26,18 @@ extern "C" int f5_qkv_quant_e4m3(const void* qkv, int64_t ld_qkv, void* qk8, int
   p.vt_ld = vt_ld;
   p.scale = qkv_scale;
   p.B = batch; p.N = frames; p.H = heads;
+  p.kv_len = kv_len;
   p.prof = ps.slot;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   F5_CHECK_CUDA(launch_kernel(qkv_quant_e4m3_kernel, dim3(cdiv(frames, 128), heads, batch), dim3(256), 0, stream, p));
   F5_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+
+// the ABI 2.001 entry: every key below frames is valid
+extern "C" int f5_qkv_quant_e4m3(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8, int64_t vt_ld,
+                                 float* qkv_scale, int32_t batch, int32_t frames, int32_t heads, void* stream) {
+  return f5_qkv_quant_e4m3_masked(qkv, ld_qkv, qk8, ld_qk8, vt8, vt_ld, qkv_scale, batch, frames, heads, nullptr, stream);
 }
 
 extern "C" int f5_attention_fwd_fp8(const void* qk8, int64_t ld_qk8, const void* vt8, int64_t vt_ld,

@@ -53,12 +53,14 @@ struct QkvQuantParams {
   // scale of its 128-key tile)
   float* scale;
   int B, N, H;
+  const int* kv_len;         // [B] valid keys per utterance, or null (= N): clamped as attn_fp8_kernel clamps it
   unsigned long long* prof;  // in-graph timing slot (ptx.cuh prof_stamp_*), or null
 };
 
 // grid (roundup(N, 128) / 128, H, B), 256 threads: one 128-key tile x (q, k, v) of one head; 8 threads per
 // (row, unit), 12 (row, unit) tasks per thread.  The bf16 rows are read once and kept in registers while the tile's k
-// and v amax is reduced through shared memory.
+// and v amax is reduced through shared memory.  Keys at or beyond kv_len are read as zero: they do not move the tile's
+// amax (a masked key must not set the scale of the valid keys beside it) and get zero K and V codes.
 __global__ void __launch_bounds__(256) qkv_quant_e4m3_kernel(const QkvQuantParams p) {
   __shared__ uint32_t stage[64 * 33];   // V^T block [d][128 key positions], row pitch 132 B (2-way store conflicts)
   __shared__ uint32_t tile_amax[2];     // k, v: fp32 bits of a non-negative (or NaN) amax, ordered as unsigned
@@ -69,6 +71,8 @@ __global__ void __launch_bounds__(256) qkv_quant_e4m3_kernel(const QkvQuantParam
   const int tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int t8 = threadIdx.x & 7, lane = threadIdx.x & 31;
   const size_t R = (size_t)p.B * p.N;
+  int kv_len = p.kv_len ? p.kv_len[b] : p.N;
+  kv_len = min(max(kv_len, 1), p.N);
   uint8_t* st8 = reinterpret_cast<uint8_t*>(stage);
   // task it: unit u = it / 4 (0 q, 1 k, 2 v: uniform per iteration), key (it % 4) * 32 + threadIdx.x / 8
   uint4 raw[12];
@@ -76,7 +80,8 @@ __global__ void __launch_bounds__(256) qkv_quant_e4m3_kernel(const QkvQuantParam
   for (int it = 0; it < 12; ++it) {
     const int n = tile * 128 + (it & 3) * 32 + (threadIdx.x >> 3);
     const int col = (it >> 2) * p.H * 64 + h * 64 + 8 * t8;
-    raw[it] = n < p.N ? *reinterpret_cast<const uint4*>(p.qkv + ((size_t)b * p.N + n) * p.ld_qkv + col)
+    const int end = it < 4 ? p.N : kv_len;   // q: every row; k, v: the valid keys
+    raw[it] = n < end ? *reinterpret_cast<const uint4*>(p.qkv + ((size_t)b * p.N + n) * p.ld_qkv + col)
                       : make_uint4(0u, 0u, 0u, 0u);
   }
   auto unpack = [](const uint4& r, float (&x)[8]) {
@@ -134,10 +139,11 @@ __global__ void __launch_bounds__(256) qkv_quant_e4m3_kernel(const QkvQuantParam
     if (u < 2) {
       if (valid) *reinterpret_cast<uint2*>(p.qk8 + row * p.ld_qk8 + u * p.H * 64 + h * 64 + 8 * t8) = make_uint2(c0, c1);
     } else {
-      // padding keys (n >= N) are written as zero codes: 0x7F is an e4m3 NaN, and 0 * NaN would pass the mask
+      // padding keys (n >= N) and masked keys (n >= kv_len, read as zero) have zero codes: 0x7F is an e4m3 NaN, and
+      // 0 * NaN would pass the mask
       const int pos = (key & ~31) + fp8_vt_pos(key & 31);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) st8[(8 * t8 + i) * 132 + pos] = valid ? (uint8_t)(((i < 4 ? c0 : c1) >> (8 * (i & 3))) & 0xFF) : 0;
+      for (int i = 0; i < 8; ++i) st8[(8 * t8 + i) * 132 + pos] = n < kv_len ? (uint8_t)(((i < 4 ? c0 : c1) >> (8 * (i & 3))) & 0xFF) : 0;
     }
   }
   __syncthreads();

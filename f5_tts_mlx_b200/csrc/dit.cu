@@ -19,8 +19,8 @@ extern "C" int f5_attention_fwd_e4m3(const void*, int64_t, void*, int64_t, int32
                                      int32_t, const int32_t*, void*);
 extern "C" int f5_attention_fwd_e4m3_scaled(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
                                             int32_t, const int32_t*, float*, void*);
-extern "C" int f5_qkv_quant_e4m3(const void*, int64_t, void*, int64_t, void*, int64_t, float*, int32_t, int32_t,
-                                 int32_t, void*);
+extern "C" int f5_qkv_quant_e4m3_masked(const void*, int64_t, void*, int64_t, void*, int64_t, float*, int32_t,
+                                        int32_t, int32_t, const int32_t*, void*);
 extern "C" int f5_attention_fwd_fp8(const void*, int64_t, const void*, int64_t, const float*, void*, int64_t, int32_t,
                                     int32_t, int32_t, int32_t, const int32_t*, float*, void*);
 
@@ -274,9 +274,9 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
     }
     if (mode.attn8) {
       const int64_t vt_ld = (int64_t)cdiv(N, 128) * 128;
-      const int32_t* kv_len = b->seq_len ? b->seq_len : b->valid_len;
-      if (int e = f5_qkv_quant_e4m3(b->qkv_bf16, 3 * D, b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, BU, N,
-                                    w->heads, st))
+      const int32_t* kv_len = b->seq_len ? b->seq_len : b->valid_len;   // the pass and the attention mask alike
+      if (int e = f5_qkv_quant_e4m3_masked(b->qkv_bf16, 3 * D, b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, BU,
+                                           N, w->heads, kv_len, st))
         return e;
       if (int e = f5_attention_fwd_fp8(b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, b->c_bf16, D, BU, N, w->heads,
                                        64, kv_len, b->attn_scale, st))

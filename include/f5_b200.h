@@ -168,11 +168,18 @@ int f5_attention_fwd_e4m3_scaled(const void* qkv, int64_t ld_qkv, void* out, int
  *                        in [frames, roundup(frames, 128)) (vt_ld bytes, multiple of 16, >= roundup(frames, 128)), and
  *                        qkv_scale fp32 [3*heads][batch*frames]: q head h -> unit h, k head h -> heads + h, v head h ->
  *                        2*heads + h (the scale rule of f5_gemm_args.a_scale, applied to the bf16 values; every k and v row holds
- *                        the scale of its 128-key tile).
+ *                        the scale of its 128-key tile).  Every key below frames is valid.
+ * f5_qkv_quant_e4m3_masked (ABI 2.002): the same with kv_len int32 [batch] (NULL = frames), the valid keys as
+ *                        f5_attention_fwd_fp8 takes them: keys at or beyond kv_len[b] do not enter their tile's k or v
+ *                        amax and get zero K and V codes; a tile without a valid key has scale 1.  Pass the
+ *                        attention's kv_len, so that masked keys cannot move the valid keys' scales.
  * f5_attention_fwd_fp8 : attention on those operands; out / scale_out as f5_attention_fwd_e4m3_scaled.
  * Pointers 16-byte aligned. */
 int f5_qkv_quant_e4m3(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8, int64_t vt_ld,
                       float* qkv_scale, int32_t batch, int32_t frames, int32_t heads, void* stream);
+int f5_qkv_quant_e4m3_masked(const void* qkv, int64_t ld_qkv, void* qk8, int64_t ld_qk8, void* vt8, int64_t vt_ld,
+                             float* qkv_scale, int32_t batch, int32_t frames, int32_t heads, const int32_t* kv_len,
+                             void* stream);
 int f5_attention_fwd_fp8(const void* qk8, int64_t ld_qk8, const void* vt8, int64_t vt_ld, const float* qkv_scale,
                          void* out, int64_t ld_out, int32_t batch, int32_t frames, int32_t heads, int32_t head_dim,
                          const int32_t* kv_len, float* scale_out, void* stream);

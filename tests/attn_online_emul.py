@@ -166,17 +166,19 @@ def online_softmax(qc, sq, kc, sk, vc, sv, kv_len, kind, *, reverse=False, flip=
     return O, beta
 
 
-def operands(qkv: torch.Tensor, B: int, N: int, H: int, kind: str):
+def operands(qkv: torch.Tensor, B: int, N: int, H: int, kind: str, kv_len=None):
     """bf16 qkv [B N, 3 H 64] -> (qc, sq, kc, sk, vc, sv) for online_softmax: the bf16 values with unit scales, or the
-    quantise pass's e4m3 codes and scales (the host rule, restated in fp8_attn_emul)."""
+    quantise pass's e4m3 codes and scales (the host rule, restated in fp8_attn_emul), with the keys at or beyond
+    kv_len [B] (None: N) out of their tiles' scales."""
     import fp8_attn_emul as A
     q, k, v = [t.reshape(B, N, H, 64).permute(0, 2, 1, 3) for t in qkv.double().split(H * 64, dim=1)]
     if kind == "bf16":
         ones = torch.ones(B, H, (N + TILE - 1) // TILE, dtype=torch.float64)
         return q, torch.ones(B, H, N, dtype=torch.float64), k, ones, v, ones
+    mask = None if kv_len is None else torch.arange(N)[None] < kv_len.cpu().long()[:, None]
     qc, sq = A.q_heads(q)
-    kc, sk = A.q_tiles(k)
-    vc, sv = A.q_tiles(v)
+    kc, sk = A.q_tiles(k, mask)
+    vc, sv = A.q_tiles(v, mask)
     return qc, sq[..., 0], kc, sk[:, :, ::TILE, 0], vc, sv[:, :, ::TILE, 0]
 
 

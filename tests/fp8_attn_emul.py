@@ -33,14 +33,18 @@ def q_heads(x: torch.Tensor):
     return E._quant(x.float(), s).double(), s.double()
 
 
-def q_tiles(x: torch.Tensor):
+def q_tiles(x: torch.Tensor, mask=None):
     """Per-(utterance, head, 128-key tile) block-scaled e4m3 of [b, h, n, 64]: (codes as float64, scales [b, h, n, 1],
-    every key carrying its tile's scale)."""
+    every key carrying its tile's scale).  mask [b, n] bool or None: masked keys are zero, so they neither move their
+    tile's amax nor carry a code (the quantise pass reads keys at or beyond kv_len as zero)."""
     b, h, n, _ = x.shape
+    x = x.float()
+    if mask is not None:
+        x = torch.where(mask.bool().to(x.device)[:, None, :, None], x, torch.zeros((), device=x.device))
     pad = (-n) % TILE
-    a = F.pad(x.float().abs(), (0, 0, 0, pad)).reshape(b, h, (n + pad) // TILE, TILE * 64).amax(-1)
+    a = F.pad(x.abs(), (0, 0, 0, pad)).reshape(b, h, (n + pad) // TILE, TILE * 64).amax(-1)
     s = E.block_scale(a).repeat_interleave(TILE, -1)[..., :n, None]
-    return E._quant(x.float(), s).double(), s.double()
+    return E._quant(x, s).double(), s.double()
 
 
 def attention_fp8(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask, heads_per_chunk: int = 4) -> torch.Tensor:
@@ -48,8 +52,8 @@ def attention_fp8(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask, heads
     The float64 scores are formed `heads_per_chunk` heads at a time (a [b, h, n, n] tensor is 8 GB at n = 5625), on
     the GPU when there is one (the result returns to q's device)."""
     qc, sq = q_heads(q)
-    kc, sk = q_tiles(k)
-    vc, sv = q_tiles(v)
+    kc, sk = q_tiles(k, mask)
+    vc, sv = q_tiles(v, mask)
     b, h, n, _ = q.shape
     dev = "cuda" if torch.cuda.is_available() else "cpu"
     valid = (mask.bool() if mask is not None else torch.ones(b, n, dtype=torch.bool)).to(dev)

@@ -21,7 +21,7 @@ def emulate(ops, kv, **kw):
 def random_case():
     qkv = M.make_qkv("random", B, N, H, seed=3)
     kv = torch.tensor([N, M.KV_LEN[N]])
-    ops = M.operands(qkv, B, N, H, "fp8")
+    ops = M.operands(qkv, B, N, H, "fp8", kv)
     M.assert_exact_logits(ops[0], ops[2], "fp8")
     return ops, kv, emulate(ops, kv)
 
@@ -30,7 +30,7 @@ def random_case():
 def tail_last_case():
     qkv = M.make_qkv("tail_last", B, N, H, seed=4)
     kv = torch.tensor([N, M.KV_LEN[N]])
-    ops = M.operands(qkv, B, N, H, "fp8")
+    ops = M.operands(qkv, B, N, H, "fp8", kv)
     M.assert_exact_logits(ops[0], ops[2], "fp8")
     return ops, kv, emulate(ops, kv)
 

@@ -97,6 +97,27 @@ def test_emulated_attention_matches_float64_on_exact_operands():
     assert ((got - want).abs() <= 2.0 ** -4 * (torch.softmax(s, -1) @ v.double().abs()) + 1e-3).all()
 
 
+def test_emulated_tile_scales_ignore_masked_keys():
+    """q_tiles with a mask: keys beyond kv_len (here +-3e4, 2^15 times the valid ones) neither set their tile's scale
+    nor carry a code, so the valid keys quantise as if those keys were zero, and attention_fp8 keeps its bits."""
+    import fp8_attn_emul as A
+    g = torch.Generator().manual_seed(1)
+    B, H, N = 2, 2, 300
+    lens = torch.tensor([300, 201])
+    mask = torch.arange(N)[None] < lens[:, None]
+    q, k, v = [torch.randn(B, H, N, 64, generator=g).bfloat16().float() for _ in range(3)]
+    poison = 3e4 * (torch.randint(0, 2, (B, H, N, 64), generator=g) * 2 - 1).float()
+    k2 = torch.where(mask[:, None, :, None], k, poison)
+    v2 = torch.where(mask[:, None, :, None], v, -poison)
+    zero = lambda t: torch.where(mask[:, None, :, None], t, torch.zeros(()))
+    for a, b in ((k, k2), (v, v2)):
+        c1, s1 = A.q_tiles(zero(a))
+        c2, s2 = A.q_tiles(b, mask)
+        assert torch.equal(c1, c2) and torch.equal(s1, s2)
+        assert not torch.equal(A.q_tiles(b)[1], s2)                 # without the mask the poison sets the scales
+    assert torch.equal(A.attention_fp8(q, k, v, mask), A.attention_fp8(q, k2, v2, mask))
+
+
 def test_fp8_attention_needs_the_block_mode():
     from f5_tts_mlx_b200 import DiT
     kw = dict(dim=256, depth=1, heads=4, text_dim=64, device="cpu")

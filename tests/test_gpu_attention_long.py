@@ -124,7 +124,7 @@ def test_attention_online_softmax_emulated(case, N, kind):
     rounds to.  The long tail also prints its drift from the float64 softmax and stays within fp8_attention_bound."""
     qkv = M.make_qkv(case, B, N, H, seed=N + len(case))
     kv = torch.tensor([N, M.KV_LEN[N]], dtype=torch.int32)
-    ops = M.operands(qkv, B, N, H, kind)
+    ops = M.operands(qkv, B, N, H, kind, kv)
     M.assert_exact_logits(ops[0], ops[2], kind)
     O, beta = M.online_softmax(*[t.to(DEV) for t in ops], kv.to(DEV), kind)
     what = f"online softmax {kind} {case} N={N}"

@@ -28,22 +28,29 @@ def _npad(n):
     return (n + 127) // 128 * 128
 
 
-def run_quant(qkv, B, N, H):
-    """f5_qkv_quant_e4m3 into guarded buffers: (qk [R, 2D], vt [B*D, Npad], scales [3H, R])."""
+def run_quant(qkv, B, N, H, kv=None):
+    """The quantise pass into guarded buffers: f5_qkv_quant_e4m3 (every key valid) when kv is None, else
+    f5_qkv_quant_e4m3_masked with kv (device int32 [B] valid keys).  Returns (qk [R, 2D], vt [B*D, Npad],
+    scales [3H, R])."""
     D, R = H * 64, B * N
     qk = Guarded(R, 2 * D, torch.uint8, DEV)
     vt = Guarded(B * D, _npad(N), torch.uint8, DEV)
     sc = Guarded(3 * H, R, torch.float32, DEV, lr=False)
-    L = _lib()
-    L.check(L.load().f5_qkv_quant_e4m3(qkv.data_ptr(), qkv.stride(0), qk.view.data_ptr(), qk.view.stride(0),
-                                       vt.view.data_ptr(), vt.view.stride(0), sc.view.data_ptr(), B, N, H, _stream()))
+    lib = _lib().load()
+    args = (qkv.data_ptr(), qkv.stride(0), qk.view.data_ptr(), qk.view.stride(0), vt.view.data_ptr(), vt.view.stride(0),
+            sc.view.data_ptr(), B, N, H)
+    if kv is None:
+        _lib().check(lib.f5_qkv_quant_e4m3(*args, _stream()))
+    else:
+        _lib().check(lib.f5_qkv_quant_e4m3_masked(*args, kv.data_ptr(), _stream()))
     return qk, vt, sc
 
 
 def run_attention(qkv, B, N, H, kv):
-    """quantise pass + f5_attention_fwd_fp8: (dequantised output [R, D] float32, out guard, scale guard)."""
+    """quantise pass + f5_attention_fwd_fp8, both with kv_len kv: (dequantised output [R, D] float32, out guard, scale
+    guard)."""
     D, R = H * 64, B * N
-    qk, vt, sc = run_quant(qkv, B, N, H)
+    qk, vt, sc = run_quant(qkv, B, N, H, kv)
     out = Guarded(R, D, torch.uint8, DEV)
     so = Guarded(H, R, torch.float32, DEV, lr=False)
     L = _lib()
@@ -66,10 +73,11 @@ def expected_vt(vcodes: torch.Tensor, N: int) -> torch.Tensor:
 
 
 # ---------------------------------------------------------------- the quantise pass
-def expected_codes(qkv: torch.Tensor, B: int, N: int, H: int):
+def expected_codes(qkv: torch.Tensor, B: int, N: int, H: int, kv_len=None):
     """The host rule applied to the bf16 qkv: q per (row, head), k and v per (utterance, head, 128-key tile)
-    (weights.quantize_e4m3_blocks with one block spanning the tile's rows).  Returns codes uint8 [R, 3D] and scales
-    [3H, R], every key carrying its tile's scale."""
+    (weights.quantize_e4m3_blocks with one block spanning the tile's rows), the keys at or beyond kv_len [B] (None: N,
+    clamped to [1, N] as the kernels do) read as zero.  Returns codes uint8 [R, 3D] and scales [3H, R], every key
+    carrying its tile's scale."""
     from f5_tts_mlx_b200.weights import E4M3_MAX, e4m3_block_scale, quantize_e4m3_blocks
     D, T = H * 64, (N + 127) // 128
     x = qkv.float()
@@ -77,8 +85,12 @@ def expected_codes(qkv: torch.Tensor, B: int, N: int, H: int):
     scales = torch.empty(3 * H, B * N)
     codes[:, :D], sq = quantize_e4m3_blocks(x[:, :D], 64)
     scales[:H] = sq.T
-    # k and v: [B, T, 128, 2, H, 64] with the padding keys zero (they do not move a tile's amax)
-    kv = torch.nn.functional.pad(x[:, D:].reshape(B, N, 2 * D), (0, 0, 0, T * 128 - N)).reshape(B, T, 128, 2, H, 64)
+    # k and v: [B, T, 128, 2, H, 64] with the padding and masked keys zero (they do not move a tile's amax)
+    kvx = x[:, D:].reshape(B, N, 2 * D)
+    if kv_len is not None:
+        valid = torch.arange(N)[None] < kv_len.cpu().long().clamp(1, N)[:, None]
+        kvx = torch.where(valid[..., None], kvx, torch.zeros(()))
+    kv = torch.nn.functional.pad(kvx, (0, 0, 0, T * 128 - N)).reshape(B, T, 128, 2, H, 64)
     s = e4m3_block_scale(kv.abs().amax(dim=(2, 5)))                                  # [B, T, 2, H]
     q = (kv * (1.0 / s)[:, :, None, :, :, None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
     codes[:, D:] = q.view(torch.uint8).reshape(B, T * 128, 2 * D)[:, :N].reshape(B * N, 2 * D)
@@ -87,12 +99,24 @@ def expected_codes(qkv: torch.Tensor, B: int, N: int, H: int):
     return codes, scales
 
 
-@pytest.mark.parametrize("N", [129, 300, 937, 5625, 8192])
-def test_quantise_pass_bitwise(N):
+_QUANT_N = [129, 300, 937, 5625, 8192]
+
+
+@pytest.mark.parametrize("N,ragged", [(n, False) for n in _QUANT_N] + [(n, True) for n in _QUANT_N],
+                         ids=[str(n) for n in _QUANT_N] + [f"{n}-ragged" for n in _QUANT_N])
+def test_quantise_pass_bitwise(N, ragged):
     """Codes and scales of Q (per row and head) and of K and V (per 128-key tile and head) equal the host rule on the
     bf16 input; V^T holds the transposed V codes in the host key order, zero codes on the padding keys; guard bands
-    untouched.  B = 3, H = 4 up to N = 937; B = 2, H = 16 at 60 s (N = 5625) and max_duration (8192)."""
+    untouched.  B = 3, H = 4 up to N = 937; B = 2, H = 16 at 60 s (N = 5625) and max_duration (8192).
+    ragged: B = 4 with kv_len = (N, ending inside a key tile, ending at a multiple of 128, 1) and every row at or
+    beyond kv_len +-3e4: those keys do not move their tile's k and v scales (the valid keys keep the codes they would
+    have without them) and have zero K and V codes; Q is quantised on every row."""
     B, H = (3, 4) if N < 1000 else (2, 16)
+    kv = None
+    if ragged:
+        B = 4
+        mid = N // 2 + 5 if (N // 2 + 5) % 128 else N // 2 + 6
+        kv = torch.tensor([N, mid, (N - 1) // 128 * 128, 1], dtype=torch.int32)
     D, R = H * 64, B * N
     g = torch.Generator().manual_seed(N)
     x = torch.randn(R, 3 * D, generator=g) * torch.pow(2.0, torch.randint(-12, 13, (R, 3 * H), generator=g).float()
@@ -100,10 +124,14 @@ def test_quantise_pass_bitwise(N):
     x[::17, :64] = 0                                              # all-zero units: scale 1
     x[5, 2 * D + 64:2 * D + 128] = 3e4                            # beyond 448
     x[N:N + 128, D + 64:D + 128] = 0                              # an all-zero k tile of utterance 1
+    if ragged:
+        for b in range(B):
+            rows = slice(b * N + int(kv[b]), (b + 1) * N)
+            x[rows] = 3e4 * (torch.randint(0, 2, x[rows].shape, generator=g) * 2 - 1)
     qkv = x.bfloat16()
-    qk, vt, sc = run_quant(qkv.to(DEV), B, N, H)
+    qk, vt, sc = run_quant(qkv.to(DEV), B, N, H, kv.to(DEV) if kv is not None else None)
     torch.cuda.synchronize()
-    codes, scales = expected_codes(qkv, B, N, H)
+    codes, scales = expected_codes(qkv, B, N, H, kv)
     assert_exact(qk.view.cpu(), codes[:, :2 * D].contiguous(), attn_tiles(N), "q|k codes")
     assert_exact(sc.view.cpu(), scales, lambda r, c: f"unit {r} row {c}", "scales")
     vt_got = vt.view.cpu()
@@ -210,7 +238,7 @@ def test_fp8_attention_random_within_bound():
     qkv = x.bfloat16()
     kv = torch.tensor([300, 201], dtype=torch.int32)
     deq, out, so = run_attention(qkv.to(DEV), B, N, H, kv.to(DEV))
-    codes, scales = expected_codes(qkv, B, N, H)
+    codes, scales = expected_codes(qkv, B, N, H, kv)
     dq = (codes.view(F8).float().reshape(B * N, 3 * H, 64) * scales.T[..., None]).reshape(B * N, 3 * D)
     split = lambda t: t.reshape(B, N, H, 64).permute(0, 2, 1, 3)
     q, k, v = split(dq[:, :D]), split(dq[:, D:2 * D]), split(dq[:, 2 * D:])
