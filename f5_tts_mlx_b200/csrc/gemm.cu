@@ -198,7 +198,9 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
     uint32_t box[2] = {kbox, (uint32_t)bn};
     if (int e = (ab8 ? make_tmap_u8 : make_tmap_bf16)(&tb, a->w, 2, dims, str, box)) return e;
   }
-  dim3 grid(cdiv(a->n, bn), batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128), 1);
+  // persistent: one CTA per SM (at most one per tile), each walking the tiles t = blockIdx.x, + gridDim.x, ...
+  const int tiles = cdiv(a->n, bn) * (batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128));
+  dim3 grid(std::min(tiles, sm_count()), 1, 1);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const bool rope = a->rope != nullptr;
   if (scaled) {

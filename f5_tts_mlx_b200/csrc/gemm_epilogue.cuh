@@ -1,5 +1,5 @@
 // Fused GEMM epilogue of the wgmma GEMM (gemm_sm90.cuh): one thread owns one output row and 32 consecutive
-// accumulator columns, read from the fp32 accumulator tile the consumer warpgroups left in shared memory.
+// accumulator columns, read from the fp32 accumulator tile the consumer warpgroup left in shared memory.
 #pragma once
 #include "ptx.cuh"
 
@@ -172,34 +172,39 @@ __device__ __forceinline__ void epi_load_resid(const GemmParams& p, int row, int
 // (half-sector writes 4 KB apart).  So every chunk (128 rows x 32 columns) is written to shared memory in the
 // layout of a swizzled TMA box (fp32: 128-byte rows, SWIZZLE_128B; bf16: 64-byte rows, SWIZZLE_64B — the XOR patterns
 // below are exactly those) and ONE thread hands it to the TMA unit (cp.async.bulk.tensor store), which also clips
-// rows / columns outside the matrix.  Two staging buffers alternate; per chunk one named barrier (128 threads).
+// rows / columns outside the matrix.  The fp32 accumulator tile is itself BN / 32 such fp32 boxes (16 KB each), so an
+// fp32 chunk is written back in place over the accumulator values its thread has just read (its own row) and stored
+// from there; bf16 / e4m3 chunks, and the second output, go to two alternating 8 KB staging buffers.  Per chunk one
+// named barrier (128 threads).
 struct EpiStage {
-  uint8_t* buf;            // 2 x 16 KB staging of this group (1024-byte aligned)
-  uint8_t* buf2;           // staging of the second (bf16) output: 2 x 8 KB (buf2_par = 8192) or 1 x 8 KB (buf2_par = 0)
-  int buf2_par;
-  int et;                  // epilogue thread 0..127 of the group; thread 0 issues the TMA stores
+  uint8_t* acc;            // the tile's fp32 accumulator boxes: BN / 32 x (128 rows x 128 bytes, SWIZZLE_128B), 1024-aligned
+  uint8_t* stg;            // 2 x 8 KB staging of the bf16 / e4m3 output, or of the second output (1024-aligned)
+  int et;                  // epilogue thread 0..127 of the warpgroup; thread 0 issues the TMA stores
   int r;                   // this thread's row inside the tile
-  int bar_id;              // named barrier of this group of 4 epilogue warps (1 + group)
+  int bar_id;              // named barrier of the epilogue warpgroup
   const CUtensorMap* map_out;   // (cols, rows per utterance, utterances) of `out` / `out2`
   const CUtensorMap* map_out2;
   int c1, c2;              // tensor-map coordinates of tile row 0: row inside the utterance, utterance
-  int par_base;            // staging buffer of a chunk = par_base ^ HALF (set by the drain loops)
   int out_fp8;             // primary output as e4m3 (GemmParams::out_fp8)
   float mu_r, rstd;        // fused-LN consumer mode: this thread's row statistics ((0, 1) otherwise)
 };
 
-// `w2`: the chunk's second output (bf16, 4 x uint4 per row) or nullptr
-// `w2_fp8`: the second output is e4m3 — 32-byte rows, SWIZZLE_32B (16-byte chunk index ^ bit 7 of the row offset)
+// this thread's row of a 128 x 32 fp32 box (SWIZZLE_128B: 16-byte piece j of row r at (j ^ (r & 7)) * 16)
+__device__ __forceinline__ void epi_stage_f32(uint8_t* buf, int r, const float (&v)[32]) {
+  uint8_t* mine = buf + r * 128;
+  const int sw = r & 7;
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    *reinterpret_cast<float4*>(mine + ((j ^ sw) * 16)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+}
+
+// chunk `ch` (columns [32 ch, 32 ch + 32) of the tile) of `out`, with its second output `w2` (bf16, 4 x uint4 per row,
+// or e4m3 when `w2_fp8`: 32-byte rows, SWIZZLE_32B = 16-byte piece index ^ bit 7 of the row offset) or nullptr
 template <bool OUT_BF16>
-__device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiStage& st, int par, int col0,
+__device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiStage& st, int ch, int col0,
                                               const uint4* w2 = nullptr, bool w2_fp8 = false) {
-  uint8_t* buf = st.buf + par * 16384;
-  uint8_t* buf2 = st.buf2 + par * st.buf2_par;
-  if (w2 != nullptr && st.buf2_par == 0) {
-    // one staging buffer for the second output: the previous chunk's store must have read it
-    if (st.et == 0) tma_store_wait_read<0>();
-    asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
-  }
+  uint8_t* box = st.acc + ch * 16384;
+  uint8_t* buf = st.stg + (ch & 1) * 8192;
   if (OUT_BF16 && st.out_fp8) {
     uint8_t* mine = buf + st.r * 32;           // e4m3: 32-byte rows, SWIZZLE_32B
     const int sw = (st.r >> 2) & 1;
@@ -219,20 +224,16 @@ __device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiSta
           make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
                      pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
   } else {
-    uint8_t* mine = buf + st.r * 128;
-    const int sw = st.r & 7;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<float4*>(mine + ((j ^ sw) * 16)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+    epi_stage_f32(box, st.r, v);
   }
-  if (w2 != nullptr) {
+  if (w2 != nullptr) {   // fp32 `out` only: the staging buffers are free for the second output
     if (w2_fp8) {
-      uint8_t* mine2 = buf2 + st.r * 32;
+      uint8_t* mine2 = buf + st.r * 32;
       const int sw2 = (st.r >> 2) & 1;
 #pragma unroll
       for (int j = 0; j < 2; ++j) *reinterpret_cast<uint4*>(mine2 + ((j ^ sw2) * 16)) = w2[j];
     } else {
-      uint8_t* mine2 = buf2 + st.r * 64;
+      uint8_t* mine2 = buf + st.r * 64;
       const int sw2 = (st.r >> 1) & 3;
 #pragma unroll
       for (int j = 0; j < 4; ++j) *reinterpret_cast<uint4*>(mine2 + ((j ^ sw2) * 16)) = w2[j];
@@ -244,24 +245,16 @@ __device__ __forceinline__ void epi_store_tma(const float (&v)[32], const EpiSta
   if (st.et == 0) tma_store_wait_read<0>();
   asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
   if (st.et == 0) {
-    tma_store_3d(st.map_out, buf, col0, st.c1, st.c2);
-    if (w2 != nullptr) tma_store_3d(st.map_out2, buf2, col0, st.c1, st.c2);
+    tma_store_3d(st.map_out, OUT_BF16 ? buf : box, col0, st.c1, st.c2);
+    if (w2 != nullptr) tma_store_3d(st.map_out2, buf, col0, st.c1, st.c2);
     tma_store_commit();
   }
 }
 
 // Block-scaled e4m3 output of one 64-column unit (the unit's scale needs both chunks, so it is quantised and stored once
-// chunk B is done).  Chunk A is not held in registers: its fp32 values wait in the fp32 staging buffer of chunk A
-// (epi_store_tma's 128-byte SWIZZLE_128B rows at st.buf), written there by HALF 0 — as the staged fp32 `out` store of
-// the producer form, or, for the e4m3 primary output, by this thread alone (its own row: no barrier) — and are read
-// back by the same thread in HALF 1.
-__device__ __forceinline__ void epi_stage_f32(uint8_t* buf, int r, const float (&v)[32]) {
-  uint8_t* mine = buf + r * 128;
-  const int sw = r & 7;
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    *reinterpret_cast<float4*>(mine + ((j ^ sw) * 16)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-}
+// chunk B is done).  Chunk A is not held in registers: its fp32 values wait in chunk A's accumulator box (its thread's
+// own row), written there by HALF 0 — as the in-place fp32 `out` store of the producer form, or, for the e4m3 primary
+// output, by this thread alone (no barrier) — and are read back by the same thread in HALF 1.
 
 // e4m3 codes of 32 values x = v * aux (aux = null: x = v), quantised as x * inv (inv = 1 / scale, exact)
 __device__ __forceinline__ void epi_quant32(const float (&v)[32], const float* aux, float inv, uint4 (&q)[2]) {
@@ -277,7 +270,7 @@ __device__ __forceinline__ void epi_quant32(const float (&v)[32], const float* a
   q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
-// the same for chunk A, read back from this thread's row of the fp32 staging buffer
+// the same for chunk A, read back from this thread's row of its fp32 box
 __device__ __forceinline__ void epi_quant32_staged(const uint8_t* buf, int r, const float* aux, float inv, uint4 (&q)[2]) {
   const uint8_t* mine = buf + r * 128;
   const int sw = r & 7;
@@ -294,18 +287,19 @@ __device__ __forceinline__ void epi_quant32_staged(const uint8_t* buf, int r, co
   q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
-// HALF 1 of a block-scaled unit: the unit's scale from the running amax (NaN propagates), written to
-// scale[colA / 64][row] (rows past the matrix write none); then the e4m3 chunks A (colA) and B (colA + 32) are staged as
-// 32-byte rows (SWIZZLE_32B), 4 KB each — of `out` (OUT_BF16: the e4m3 primary output, in the second 16 KB of st.buf,
-// chunk A's fp32 values being in the first) or of out2 (in st.buf2, with the fp32 chunk B of `out` staged as in
-// epi_store_tma) — and stored.  Each staged piece is written as soon as it is formed, so that few values are live at once.
+// HALF 1 of a block-scaled unit (chunks chA, chA + 1): the unit's scale from the running amax (NaN propagates), written
+// to scale[colA / 64][row] (rows past the matrix write none); then the e4m3 chunks A (colA) and B (colA + 32) are staged
+// as 32-byte rows (SWIZZLE_32B), 4 KB each, in the unit's 8 KB staging buffer (units alternate between the two, so a
+// unit never rewrites the buffer the previous unit's store may still read) — of `out` (OUT_BF16: the e4m3 primary
+// output) or of out2 (with the fp32 chunk B of `out` written in place in its box) — and stored.  Each staged piece is
+// written as soon as it is formed, so that few values are live at once.
 template <bool OUT_BF16>
 __device__ __forceinline__ void epi_finish_unit8(const float (&v)[32], const float* aux, float amax, float* scale,
-                                                 int M, int colA, int row, bool row_ok, const EpiStage& st) {
+                                                 int M, int colA, int row, bool row_ok, const EpiStage& st, int chA) {
   float inv;
   const float s = e4m3_block_scale(amax, inv);
   if (row_ok) scale[(size_t)(colA >> 6) * M + row] = s;
-  uint8_t* q8 = OUT_BF16 ? st.buf + 16384 : st.buf2;
+  uint8_t* q8 = st.stg + ((chA >> 1) & 1) * 8192;
   const int sw = (st.r >> 2) & 1;
   {
     uint4 q[2];
@@ -313,11 +307,11 @@ __device__ __forceinline__ void epi_finish_unit8(const float (&v)[32], const flo
 #pragma unroll
     for (int j = 0; j < 2; ++j) *reinterpret_cast<uint4*>(q8 + 4096 + st.r * 32 + ((j ^ sw) * 16)) = q[j];
   }
-  uint8_t* buf = st.buf + (st.par_base ^ 1) * 16384;
-  if constexpr (!OUT_BF16) epi_stage_f32(buf, st.r, v);
+  uint8_t* box_b = st.acc + (chA + 1) * 16384;
+  if constexpr (!OUT_BF16) epi_stage_f32(box_b, st.r, v);
   {
     uint4 q[2];
-    epi_quant32_staged(st.buf + st.par_base * 16384, st.r, aux != nullptr ? aux - 32 : nullptr, inv, q);
+    epi_quant32_staged(st.acc + chA * 16384, st.r, aux != nullptr ? aux - 32 : nullptr, inv, q);
 #pragma unroll
     for (int j = 0; j < 2; ++j) *reinterpret_cast<uint4*>(q8 + st.r * 32 + ((j ^ sw) * 16)) = q[j];
   }
@@ -325,7 +319,7 @@ __device__ __forceinline__ void epi_finish_unit8(const float (&v)[32], const flo
   if (st.et == 0) tma_store_wait_read<0>();
   asm volatile("bar.sync %0, 128;" ::"r"(st.bar_id) : "memory");
   if (st.et == 0) {
-    if constexpr (!OUT_BF16) tma_store_3d(st.map_out, buf, colA + 32, st.c1, st.c2);
+    if constexpr (!OUT_BF16) tma_store_3d(st.map_out, box_b, colA + 32, st.c1, st.c2);
     const CUtensorMap* m8 = OUT_BF16 ? st.map_out : st.map_out2;
     tma_store_3d(m8, q8, colA, st.c1, st.c2);
     tma_store_3d(m8, q8 + 4096, colA + 32, st.c1, st.c2);
@@ -333,7 +327,8 @@ __device__ __forceinline__ void epi_finish_unit8(const float (&v)[32], const flo
   }
 }
 
-// HALF: which 32-column half of a 64-column head this chunk is (static RoPE register indexing)
+// HALF: which 32-column half of a 64-column head this chunk is (static RoPE register indexing); `ch`: the chunk's index
+// in the tile (its accumulator box)
 // `unit_acc`: running (sum, sum of squares) of this thread's row over the 64-column unit (HALF 0 starts it, HALF 1
 // completes and stores it) — fused-LN producer mode only.
 // SC (block-scaled instantiations): the accumulator term is multiplied by ws_s[col] (acc_scale * w_scale); a block-scaled
@@ -342,7 +337,7 @@ template <int ACT, bool OUT_BF16, bool ROPE, int HALF, bool SC = false>
 __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float4 (&res)[8],
                                           const float* bias_s, const float* gate_s, const float* aux_s,
                                           const float2 (&cs)[ROPE ? 32 : 1], const GemmParams& p,
-                                          int col0, int row, bool row_ok, bool row_valid,
+                                          int col0, int ch, int row, bool row_ok, bool row_valid,
                                           const EpiStage& st, float2& unit_acc, const float* ws_s = nullptr,
                                           float* unit_amax = nullptr) {
   float v[32];
@@ -442,9 +437,9 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
           for (int j = 0; j < 32; ++j) amax = fmax_nan(amax, fabsf(v[j] * aux_s[j]));
           if (HALF == 0) {
             *unit_amax = amax;
-            epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0);    // the fp32 chunk A leaves now (and stays staged)
+            epi_store_tma<OUT_BF16>(v, st, ch, col0);    // the fp32 chunk A leaves now (and stays in its box)
           } else {
-            epi_finish_unit8<OUT_BF16>(v, aux_s, amax, p.out2_scale, p.M, col0 - 32, row, row_ok, st);
+            epi_finish_unit8<OUT_BF16>(v, aux_s, amax, p.out2_scale, p.M, col0 - 32, row, row_ok, st, ch - 1);
           }
           return;
         }
@@ -471,7 +466,7 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
                              pack_bf16x2(v[8 * j + 4] * s1.x, v[8 * j + 5] * s1.y), pack_bf16x2(v[8 * j + 6] * s1.z, v[8 * j + 7] * s1.w));
         }
       }
-      epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0, w2, p.out2_fp8 != 0);
+      epi_store_tma<OUT_BF16>(v, st, ch, col0, w2, p.out2_fp8 != 0);
       return;
     }
   }
@@ -482,54 +477,59 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
       for (int j = 0; j < 32; ++j) amax = fmax_nan(amax, fabsf(v[j]));
       if (HALF == 0) {
         *unit_amax = amax;
-        epi_stage_f32(st.buf + st.par_base * 16384, st.r, v);   // chunk A waits in its (own-row) fp32 staging
+        epi_stage_f32(st.acc + ch * 16384, st.r, v);   // chunk A waits in its own row of its fp32 box
       } else {
-        epi_finish_unit8<OUT_BF16>(v, nullptr, amax, p.out_scale, p.M, col0 - 32, row, row_ok, st);
+        epi_finish_unit8<OUT_BF16>(v, nullptr, amax, p.out_scale, p.M, col0 - 32, row, row_ok, st, ch - 1);
       }
       return;
     }
   }
-  epi_store_tma<OUT_BF16>(v, st, st.par_base ^ HALF, col0);   // all 128 threads of the group take part (barrier inside)
+  epi_store_tma<OUT_BF16>(v, st, ch, col0);   // all 128 threads of the warpgroup take part (barrier inside)
 }
 
-// 32 consecutive fp32 accumulator columns of this thread's row (shared memory, 16-byte aligned)
-__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&acc)[32]) {
+// the 32 fp32 accumulator columns of this thread's row in a 128 x 32 box (SWIZZLE_128B, as epi_stage_f32 writes them)
+__device__ __forceinline__ void acc_ld32(const uint8_t* box, int r, uint32_t (&acc)[32]) {
+  const uint8_t* mine = box + r * 128;
+  const int sw = r & 7;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    const float4 v = *reinterpret_cast<const float4*>(src + 4 * j);
+    const float4 v = *reinterpret_cast<const float4*>(mine + ((j ^ sw) * 16));
     acc[4 * j] = __float_as_uint(v.x); acc[4 * j + 1] = __float_as_uint(v.y);
     acc[4 * j + 2] = __float_as_uint(v.z); acc[4 * j + 3] = __float_as_uint(v.w);
   }
 }
 
-// Drains one accumulator tile of BN columns: `acc_row` = this thread's row of the shared-memory accumulator tile,
-// already offset to the group's first column.  `res0` holds the residual of the first 32 columns.
+// Drains one accumulator tile of BN columns (st.acc: its BN / 32 fp32 boxes; this thread's row st.r).  `res0` holds the
+// residual of the first 32 columns (loaded here instead in the RoPE and block-scaled forms).
 template <int BN, int ACT, bool OUT_BF16, bool ROPE, bool SC = false>
-__device__ __forceinline__ void epi_drain_tile(const float* acc_row, const float* bias_s,
-                                               const float* gate_s, const float* aux_s, const float2 (&cs)[ROPE ? 32 : 1],
-                                               float4 (&res0)[8], const GemmParams& p, int n0, int row,
-                                               bool row_ok, bool row_valid, EpiStage& st,
+__device__ __forceinline__ void epi_drain_tile(const float* bias_s, const float* gate_s, const float* aux_s,
+                                               const float2 (&cs)[ROPE ? 32 : 1], float4 (&res0)[8], const GemmParams& p,
+                                               int n0, int row, bool row_ok, bool row_valid, const EpiStage& st,
                                                const float* ws_s = nullptr) {
   float4 res1[8];
   float2 unit_acc = make_float2(0.f, 0.f);
   float unit_amax = 0.f;
-  st.par_base = 0;
 #pragma unroll 1
   for (int cc = 0; cc < BN / 64; ++cc) {
     const int colA = n0 + cc * 64, colB = colA + 32;
     uint32_t acc[32];
-    // chunk A (first half of the head): request chunk B's residual, then drain A
-    epi_load_resid(p, row, colB, row_ok, res1);
-    acc_ld32(acc_row + cc * 64, acc);
+    // chunk A (first half of the head): request chunk B's residual, then drain A.  A later unit's first residual is
+    // requested here too, not under the previous chunk B.  The RoPE and block-scaled epilogues hold more registers
+    // (the head's cos / sin, the unit's amax): they request chunk B's residual after chunk A (RoPE GEMMs get none).
+    constexpr bool kLateB = ROPE || SC;
+    if (kLateB || cc > 0) epi_load_resid(p, row, colA, row_ok, res0);
+    if constexpr (!kLateB) epi_load_resid(p, row, colB, row_ok, res1);
+    acc_ld32(st.acc + (2 * cc) * 16384, st.r, acc);
     if (colA < p.N)   // uniform per CTA
-      epi_apply<ACT, OUT_BF16, ROPE, 0, SC>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA, row,
-                                            row_ok, row_valid, st, unit_acc, SC ? ws_s + cc * 64 : nullptr, &unit_amax);
-    // chunk B: request the next unit's first residual, then drain B
-    if (cc + 1 < BN / 64) epi_load_resid(p, row, colA + 64, row_ok, res0);
-    acc_ld32(acc_row + cc * 64 + 32, acc);
+      epi_apply<ACT, OUT_BF16, ROPE, 0, SC>(acc, res0, bias_s + cc * 64, gate_s + cc * 64, aux_s + cc * 64, cs, p, colA,
+                                            2 * cc, row, row_ok, row_valid, st, unit_acc, SC ? ws_s + cc * 64 : nullptr,
+                                            &unit_amax);
+    // chunk B
+    if constexpr (kLateB) epi_load_resid(p, row, colB, row_ok, res1);
+    acc_ld32(st.acc + (2 * cc + 1) * 16384, st.r, acc);
     if (colB < p.N)
       epi_apply<ACT, OUT_BF16, ROPE, 1, SC>(acc, res1, bias_s + cc * 64 + 32, gate_s + cc * 64 + 32, aux_s + cc * 64 + 32, cs,
-                                            p, colB, row, row_ok, row_valid, st, unit_acc,
+                                            p, colB, 2 * cc + 1, row, row_ok, row_valid, st, unit_acc,
                                             SC ? ws_s + cc * 64 + 32 : nullptr, &unit_amax);
   }
 }

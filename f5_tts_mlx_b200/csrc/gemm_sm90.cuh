@@ -1,13 +1,19 @@
 // wgmma + TMA GEMM for sm_90a:  D[M,N] = epilogue( A[M,K] (bf16 or e4m3, K-major) · W[N,K]^T )
 //
-// One CTA computes one 128 x BN output tile with 384 threads (three warpgroups):
-//   warpgroup 0   TMA producer (one elected thread of warp 0): A/B k-blocks -> 128B-swizzled smem ring; the first
-//                 ring of weight tiles is requested before the PDL wait when the caller marks W as static
-//   warpgroups 1-2 consumers: warpgroup g multiplies rows [64 g, 64 g + 64) of the tile (wgmma m64nBN, fp32
-//                 accumulator in registers), keeping one MMA group in flight while the previous stage is released
-// Pipeline: smem full/empty mbarriers (TMA <-> consumers).  After the main loop the consumers write their
-// accumulators to an fp32 tile in shared memory and become the epilogue: one thread per output row, one group of
-// 128 threads per BN / kGroups columns (gemm_epilogue.cuh).
+// Persistent: min(tiles, SMs) CTAs of 384 threads (three warpgroups), one per SM; CTA c computes the 128 x BN output
+// tiles t = c, c + G, c + 2G, ... (G = gridDim.x; tile t is column tile t % tiles_n of row tile t / tiles_n, so the
+// tiles in flight at once are the first wave of the one-tile-per-CTA grid).
+//   warpgroup 0   TMA producer (one elected thread of warp 0): streams the A/B k-blocks of the CTA's tiles, tile after
+//                 tile, through one 128B-swizzled smem ring; the first ring of weight tiles is requested before the
+//                 PDL wait when the caller marks W as static
+//   warpgroups 1-2 consumers, ping-pong: local tile j of the CTA belongs to warpgroup j & 1, which multiplies all 128
+//                 rows (two wgmma m64nBN accumulators in registers) and then runs the tile's epilogue — while the other
+//                 warpgroup runs tile j + 1's MMAs
+// Pipeline: smem full/empty mbarriers (TMA <-> the consumer warpgroup reading the stage), plus two hand-over mbarriers
+// between the consumers: `mma_turn` (tile j's main loop is done: tile j + 1 may wait on the ring — the ring's phase
+// bits only tell k-blocks apart in order) and `epi_free` (tile j's epilogue has finished with the accumulator tile and
+// the staging: tile j + 1 may write them).  The accumulator tile is BN / 32 fp32 boxes of 128 rows x 32 columns in the
+// layout of the epilogue's TMA stores; the epilogue is one thread per output row (gemm_epilogue.cuh).
 //
 // The same kernel runs the 1-D convolutions of the path as implicit GEMMs: the A operand is a
 // 3-D tensor map (channels, frames, batch) and k-block kb reads the tile shifted by
@@ -35,24 +41,22 @@ struct GemmSmem {
   static constexpr int kABytes = 128 * 128;           // 128 rows x 128 bytes (64 bf16 / 128 e4m3)
   static constexpr int kBBytes = BN * 128;
   static constexpr int kStageBytes = kABytes + kBBytes;
+  // accumulator tile: BN / 32 fp32 boxes of 128 rows x 128 bytes (SWIZZLE_128B), the epilogue's fp32 TMA-store boxes
   static constexpr int kAccOffset = kStages * kStageBytes;
-  static constexpr int kAccLd = BN + 4;                // floats per accumulator row: conflict-free row-wise float4 reads
-  static constexpr int kBarOffset = kAccOffset + 128 * kAccLd * 4;
-  static constexpr int kColsOffset = (kBarOffset + 2 * kStages * 8 + 15) & ~15;   // bias_s[BN], gate_s[BN], aux_s[BN]
+  static constexpr int kAccBytes = (BN / 32) * 16384;
+  // staging of the bf16 / e4m3 outputs and of the second output: 2 x 8 KB
+  static constexpr int kStgOffset = kAccOffset + kAccBytes;
+  // full[kStages], empty[kStages], mma_turn, epi_free
+  static constexpr int kBarOffset = kStgOffset + 16384;
+  static constexpr int kColsOffset = (kBarOffset + (2 * kStages + 2) * 8 + 15) & ~15;   // bias_s[BN], gate_s[BN], aux_s[BN]
   // block-scaled instantiations also stage ws_s[BN] (the per-column weight scale)
   static constexpr int kTotal = kColsOffset + (SCALED ? 4 : 3) * BN * 4 + 1024;  // + align slack
-  // epilogue store staging reuses the (idle) operand ring: fp32/bf16 chunks at [0, 64 KB) (32 KB per group), the
-  // bf16 copy of the fused-LN producer mode at [64 KB, 96 KB) (16 KB per group, two alternating 8 KB buffers)
-  static_assert(kStages * kStageBytes >= 98304, "operand ring too small for the epilogue staging");
+  static_assert(kStageBytes % 1024 == 0, "SWIZZLE_128B tiles and boxes sit on 1024-byte boundaries");
   static_assert(kTotal <= 232448, "GEMM: shared memory over the 227 KB limit");
 };
 
-// Epilogue groups: 128 threads each (one per tile row); with 128-column tiles the two consumer warpgroups drain
-// columns [0, 64) and [64, 128) side by side.
 template <int BN>
 struct GemmEpi {
-  static constexpr int kGroups = BN >= 128 ? 2 : 1;
-  static constexpr int kCols = BN / kGroups;          // columns per group
   static constexpr int kThreads = 384;
 };
 
@@ -65,6 +69,38 @@ __device__ __forceinline__ void gemm_wgmma(float (&acc)[BN / 2], uint64_t da, ui
     if constexpr (BN == 128) wgmma_bf16_ss_n128(acc, da, db, scale_d);
     else wgmma_bf16_ss_n64(acc, da, db, scale_d);
   }
+}
+
+// Output tile t of the grid-stride walk: column tile t % tiles_n, row tile t / tiles_n (flat rows, or tiles_per_batch
+// row tiles per utterance in batched / conv mode).
+struct GemmTile {
+  int n0;             // first output column
+  int batch;          // utterance (batched mode; 0 otherwise)
+  int m_in_batch0;    // first row inside the utterance (flat mode: = row0)
+  int row0;           // first row of the flat [M, ...] matrices
+};
+__device__ __forceinline__ GemmTile gemm_tile(const GemmParams& p, int t, int bn) {
+  GemmTile g;
+  const int tiles_n = (p.N + bn - 1) / bn;
+  const int mt = t / tiles_n;
+  g.n0 = (t - mt * tiles_n) * bn;
+  if (p.tiles_per_batch > 0) {
+    g.batch = mt / p.tiles_per_batch;
+    g.m_in_batch0 = (mt - g.batch * p.tiles_per_batch) * 128;
+    g.row0 = g.batch * p.rows_per_batch + g.m_in_batch0;
+  } else {
+    g.batch = 0;
+    g.row0 = mt * 128;
+    g.m_in_batch0 = g.row0;
+  }
+  return g;
+}
+__device__ __forceinline__ int gemm_tiles(const GemmParams& p, int bn) {
+  return (p.N + bn - 1) / bn * (p.tiles_per_batch > 0 ? p.num_batches * p.tiles_per_batch : (p.M + 127) / 128);
+}
+// k-blocks per tile: always 128 bytes per row (one swizzle span), 64 bf16 or 128 e4m3 elements
+__device__ __forceinline__ int gemm_num_kb(const GemmParams& p) {
+  return p.conv_taps * (p.ab8 ? (p.k_per_tap + 127) >> 7 : (p.k_per_tap + 63) >> 6);
 }
 
 // FP8 = false instantiations have every e4m3 feature (ab8 / out_fp8 / out2_fp8 / acc_scale) folded away at compile
@@ -83,34 +119,18 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
   if constexpr (!RESID) p.resid = nullptr;
   if constexpr (!SCALED) { p.a_scale = nullptr; p.w_scale = nullptr; p.out_scale = nullptr; p.out2_scale = nullptr; }
   using S = GemmSmem<BN, kStages, SCALED>;
-  using E = GemmEpi<BN>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must sit on 1024-byte boundaries
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::kBarOffset);
   uint64_t* empty_bar = full_bar + kStages;
-  float* acc_s = reinterpret_cast<float*>(smem + S::kAccOffset);
+  uint64_t* mma_turn = empty_bar + kStages;
+  uint64_t* epi_free = mma_turn + 1;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // ---- tile coordinates ----
-  const int n0 = blockIdx.x * BN;
-  int batch = 0, m_in_batch0 = 0, row0;
-  if (p.tiles_per_batch > 0) {
-    batch = blockIdx.y / p.tiles_per_batch;
-    m_in_batch0 = (blockIdx.y % p.tiles_per_batch) * 128;
-    row0 = batch * p.rows_per_batch + m_in_batch0;
-  } else {
-    row0 = blockIdx.y * 128;
-    m_in_batch0 = row0;
-  }
-  const int kbe = p.ab8 ? 128 : 64;      // elements per k-block: always 128 bytes per row (one swizzle span)
-  const int kb_per_tap = (p.k_per_tap + kbe - 1) / kbe;
-  const int num_kb = p.conv_taps * kb_per_tap;
-
   // ---- one-time setup (overlaps the predecessor kernel under PDL) ----
-  const int cta_lin = blockIdx.y * gridDim.x + blockIdx.x;
   if (warp == 0 && elect_one()) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
@@ -118,26 +138,30 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
     if (p.out2 != nullptr) tma_prefetch_desc(&tma_out2);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 256);   // every consumer thread releases the stage it has read
+      mbar_init(&empty_bar[i], 128);   // every thread of the consumer warpgroup that read the stage releases it
     }
+    mbar_init(mma_turn, 128);
+    mbar_init(epi_free, 128);
     fence_mbar_init();
   }
-  if (warp == 1) prefetch_slice_l2(p, cta_lin, gridDim.x * gridDim.y, lane);
+  if (warp == 1) prefetch_slice_l2(p, blockIdx.x, gridDim.x, lane);
   __syncthreads();
-  // weights do not depend on the predecessor kernel: the first ring of B tiles is requested BEFORE the PDL
-  // wait, so their (possibly HBM) latency runs under the predecessor's tail
-  const int early_b = p.w_static ? min(kStages, num_kb) : 0;
+  // weights do not depend on the predecessor kernel: the first ring of the first tile's B tiles is requested BEFORE
+  // the PDL wait, so their (possibly HBM) latency runs under the predecessor's tail
+  const int early_b = p.w_static ? min(kStages, gemm_num_kb(p)) : 0;
   if (warp == 0 && elect_one()) {
+    const int n0 = gemm_tile(p, blockIdx.x, BN).n0;
     for (int kb = 0; kb < early_b; ++kb) {
       mbar_expect_tx(&full_bar[kb], S::kStageBytes);
-      tma_load_2d(smem + kb * S::kStageBytes + S::kABytes, &tma_b, &full_bar[kb], kb * kbe, n0);
+      tma_load_2d(smem + kb * S::kStageBytes + S::kABytes, &tma_b, &full_bar[kb], kb * (p.ab8 ? 128 : 64), n0);
     }
   }
   pdl_wait();   // predecessor's outputs (our A operand / residual) are complete and visible
   if (threadIdx.x == 128) prof_stamp_begin(p.prof);
 
-  // Registers move from the producer warpgroup (one thread issues TMA) to the consumers, whose epilogue holds RoPE
-  // tables and residual tiles next to the accumulator chunk: 128 x 40 + 256 x 232 = the 384 x 168 of the launch.
+  // Registers move from the producer warpgroup (one thread issues TMA) to the consumers, which hold a whole tile's
+  // accumulator (BN registers) in the main loop and RoPE tables and residual tiles in the epilogue:
+  // 128 x 40 + 256 x 232 = the 384 x 168 of the launch.
   if (warp < 4) {
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
@@ -145,160 +169,191 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
       auto produce = [&](auto ab8_tag) {
         constexpr int KBE = decltype(ab8_tag)::value ? 128 : 64;     // elements per k-block, compile-time in the loop
         // incremental stage / phase / tap bookkeeping: no division in the loop
-        int s = 0, tap = 0, kc = 0;
+        const int kb_per_tap = (p.k_per_tap + KBE - 1) / KBE, num_kb = p.conv_taps * kb_per_tap, tiles = gemm_tiles(p, BN);
+        int s = 0;
         uint32_t ph = 1;
         uint8_t* sa = smem;
-        const int a_col0 = p.conv_grouped ? n0 : 0;
-        const int a_row0 = m_in_batch0 - p.conv_pad;
-        const int a_b = p.tiles_per_batch > 0 ? batch : 0;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[s], ph);
-          if (kb >= early_b) mbar_expect_tx(&full_bar[s], S::kStageBytes);
-          tma_load_3d(sa, &tma_a, &full_bar[s], a_col0 + kc * KBE, a_row0 + tap, a_b);
-          if (kb >= early_b) tma_load_2d(sa + S::kABytes, &tma_b, &full_bar[s], kb * KBE, n0);
-          if (++s == kStages) { s = 0; ph ^= 1; sa = smem; } else { sa += S::kStageBytes; }
-          if (++kc == kb_per_tap) { kc = 0; ++tap; }
+        int early = p.w_static ? min(kStages, num_kb) : 0;   // the first tile's early weight tiles
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+          const GemmTile g = gemm_tile(p, t, BN);
+          const int a_col0 = p.conv_grouped ? g.n0 : 0;
+          const int a_row0 = g.m_in_batch0 - p.conv_pad;
+          int tap = 0, kc = 0;
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&empty_bar[s], ph);
+            if (kb >= early) mbar_expect_tx(&full_bar[s], S::kStageBytes);
+            tma_load_3d(sa, &tma_a, &full_bar[s], a_col0 + kc * KBE, a_row0 + tap, g.batch);
+            if (kb >= early) tma_load_2d(sa + S::kABytes, &tma_b, &full_bar[s], kb * KBE, g.n0);
+            if (++s == kStages) { s = 0; ph ^= 1; sa = smem; } else { sa += S::kStageBytes; }
+            if (++kc == kb_per_tap) { kc = 0; ++tap; }
+          }
+          early = 0;
         }
       };
       if (p.ab8) produce(std::true_type{});
       else produce(std::false_type{});
     }
   } else {
-    // ===================== consumers: main loop =====================
+    // ===================== consumers: ping-pong over the CTA's tiles =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-    const int wg = (threadIdx.x >> 7) - 1;          // 0: tile rows [0, 64), 1: [64, 128)
-    const int et = threadIdx.x & 127;
-    const int grp = wg;                             // epilogue group (columns [grp * kCols, (grp + 1) * kCols))
-    constexpr int BNG = E::kCols;
-    const int n0g = n0 + grp * BNG;
-    float* bias_s = reinterpret_cast<float*>(smem + S::kColsOffset) + grp * BNG;
-    float* gate_s = reinterpret_cast<float*>(smem + S::kColsOffset) + BN + grp * BNG;
-    float* aux_s = reinterpret_cast<float*>(smem + S::kColsOffset) + 2 * BN + grp * BNG;
-    float* ws_s = SCALED ? reinterpret_cast<float*>(smem + S::kColsOffset) + 3 * BN + grp * BNG : nullptr;
-    if (grp < E::kGroups) epi_stage_cols<BNG, SCALED>(p, n0g, et, bias_s, gate_s, aux_s, ws_s);   // under the main loop's loads
+    const int wg = (threadIdx.x >> 7) - 1;          // local tiles j = wg, wg + 2, ...
+    const int et = threadIdx.x & 127;               // epilogue: this thread's tile row
+    const int wr = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // accumulator fragment rows wr, wr + 8 (+ 64 h)
+    const uint32_t ring = smem_u32(smem);
+    uint8_t* acc_tile = smem + S::kAccOffset;
+    float* bias_s = reinterpret_cast<float*>(smem + S::kColsOffset);
+    float* gate_s = bias_s + BN;
+    float* aux_s = bias_s + 2 * BN;
+    float* ws_s = SCALED ? bias_s + 3 * BN : nullptr;
 
-    float acc[BN / 2];
+    // local tile j waits for tile j - 1's hand-overs: phase j - 1 of mma_turn / epi_free, parity (j - 1) & 1 = wg ^ 1
+    const uint32_t turn_par = (uint32_t)wg ^ 1u;
+#pragma unroll 1
+    for (int t = blockIdx.x + wg * gridDim.x; t < gemm_tiles(p, BN); t += 2 * gridDim.x) {
+      const int num_kb = gemm_num_kb(p);
+      const bool first = t == (int)blockIdx.x;   // j == 0
+      // the tile's first k-block in the CTA's stream: j * num_kb, j = local tile index (only t is carried across tiles)
+      const int kb0 = (t - (int)blockIdx.x) / (int)gridDim.x * num_kb;
+      int s = kb0 % kStages;
+      uint32_t ph = (uint32_t)(kb0 / kStages) & 1u;
+      if (!first) mbar_wait(mma_turn, turn_par);   // tile j - 1 has waited on all of its k-blocks
+
+      float acc[2][BN / 2];   // rows [0, 64) and [64, 128) of the tile
 #pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    auto mma_loop = [&](auto ab8_tag) {
-      constexpr bool AB8 = decltype(ab8_tag)::value;
-      const uint32_t ring = smem_u32(smem);
-      int s = 0, s_prev = 0;
-      uint32_t ph = 0;
-      if constexpr (AB8) {
-        // e4m3 wgmma accumulates with fewer mantissa bits than fp32: each k-block (128 products per output) goes to
-        // a fresh partial accumulator that is added to the fp32 accumulator on the CUDA cores
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+      auto mma_loop = [&](auto ab8_tag) {
+        constexpr bool AB8 = decltype(ab8_tag)::value;
+        if constexpr (AB8) {
+          // e4m3 wgmma accumulates with fewer mantissa bits than fp32: each k-block (128 products per output) goes to
+          // a fresh partial accumulator that is added to the fp32 accumulator on the CUDA cores, one 64-row half at a time
+          float part[BN / 2];
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sa = ring + s * S::kStageBytes, sb = ring + s * S::kStageBytes + S::kABytes;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < 4; ++k)
+                gemm_wgmma<BN, true>(part, gmma_desc_sw128(sa + h * (64 * 128) + 32 * k, 16, 1024),
+                                     gmma_desc_sw128(sb + 32 * k, 16, 1024), k != 0);
+              wgmma_commit();
+              wgmma_wait<0>();
+              wgmma_reg_fence(part);
+              if (h == 1) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+              for (int i = 0; i < BN / 2; ++i) acc[h][i] += part[i];
+            }
+            if (++s == kStages) { s = 0; ph ^= 1; }
+          }
+        } else {
+          int s_prev = 0;
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full_bar[s], ph);
+            const uint32_t sa = ring + s * S::kStageBytes, sb = ring + s * S::kStageBytes + S::kABytes;
+            wgmma_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int k = 0; k < 4; ++k)    // 4 K-steps of 16 bf16 (32 bytes) per 128-byte k-block row
+                gemm_wgmma<BN, false>(acc[h], gmma_desc_sw128(sa + h * (64 * 128) + 32 * k, 16, 1024),
+                                      gmma_desc_sw128(sb + 32 * k, 16, 1024), (kb | k) != 0);
+            wgmma_commit();
+            // the previous k-block's MMAs have retired once at most this one is in flight: release its stage
+            wgmma_wait<1>();
+            if (kb > 0) mbar_arrive(&empty_bar[s_prev]);
+            s_prev = s;
+            if (++s == kStages) { s = 0; ph ^= 1; }
+          }
+          wgmma_wait<0>();
+          wgmma_reg_fence(acc[0]);
+          wgmma_reg_fence(acc[1]);
+          mbar_arrive(&empty_bar[s_prev]);
+        }
+      };
+      // Block-scaled A: each 128-byte e4m3 k-block holds two 64-element units with their own row scales.  A unit's two
+      // k32 wgmmas go to a fresh partial that is promoted as acc = fma(part, s_a[row], acc), one 64-row half at a time.
+      // The thread's fragment rows are wr and wr + 8 of each half (acc[h][i] belongs to row 64 h + wr + 8 ((i / 2) % 2));
+      // their scales are loaded before the stage's wait, and only for rows that exist (TMA zero-fills A past the matrix
+      // or the utterance, a plain load would not).
+      auto mma_loop_scaled = [&]() {
+        const GemmTile g = gemm_tile(p, t, BN);
+        const int lim = p.tiles_per_batch > 0 ? p.rows_per_batch - g.m_in_batch0 : p.M - g.row0;   // rows that exist
+        const float* sp = p.a_scale + g.row0 + wr;
+        const size_t ld = (size_t)p.a_scale_ld;
         float part[BN / 2];
         for (int kb = 0; kb < num_kb; ++kb) {
+          float sc[2][2][2];   // [unit][half][row]
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const float* su = sp + (size_t)(2 * kb + u) * ld;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              sc[u][h][0] = 64 * h + wr < lim ? su[64 * h] : 0.f;
+              sc[u][h][1] = 64 * h + wr + 8 < lim ? su[64 * h + 8] : 0.f;
+            }
+          }
           mbar_wait(&full_bar[s], ph);
-          const uint32_t sa = ring + s * S::kStageBytes + wg * (64 * 128), sb = ring + s * S::kStageBytes + S::kABytes;
-          wgmma_fence();
+          const uint32_t sa = ring + s * S::kStageBytes, sb = ring + s * S::kStageBytes + S::kABytes;
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            gemm_wgmma<BN, true>(part, gmma_desc_sw128(sa + 32 * k, 16, 1024), gmma_desc_sw128(sb + 32 * k, 16, 1024),
-                                 k != 0);
-          wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_reg_fence(part);
-          mbar_arrive(&empty_bar[s]);
+          for (int u = 0; u < 2; ++u) {
 #pragma unroll
-          for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+            for (int h = 0; h < 2; ++h) {
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < 2; ++k)
+                gemm_wgmma<BN, true>(part, gmma_desc_sw128(sa + h * (64 * 128) + 64 * u + 32 * k, 16, 1024),
+                                     gmma_desc_sw128(sb + 64 * u + 32 * k, 16, 1024), k != 0);
+              wgmma_commit();
+              wgmma_wait<0>();
+              wgmma_reg_fence(part);
+              if (u == 1 && h == 1) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+              for (int i = 0; i < BN / 2; ++i) acc[h][i] = fmaf(part[i], sc[u][h][(i >> 1) & 1], acc[h][i]);
+            }
+          }
           if (++s == kStages) { s = 0; ph ^= 1; }
         }
+      };
+      if constexpr (SCALED) {
+        if (p.ab8 && p.a_scale != nullptr) mma_loop_scaled();
+        else if (p.ab8) mma_loop(std::true_type{});
+        else mma_loop(std::false_type{});
       } else {
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[s], ph);
-          const uint32_t sa = ring + s * S::kStageBytes + wg * (64 * 128), sb = ring + s * S::kStageBytes + S::kABytes;
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k)    // 4 K-steps of 16 bf16 (32 bytes) per 128-byte k-block row
-            gemm_wgmma<BN, false>(acc, gmma_desc_sw128(sa + 32 * k, 16, 1024), gmma_desc_sw128(sb + 32 * k, 16, 1024),
-                                  (kb | k) != 0);
-          wgmma_commit();
-          // the previous k-block's MMAs have retired once at most this one is in flight: release its stage
-          wgmma_wait<1>();
-          if (kb > 0) mbar_arrive(&empty_bar[s_prev]);
-          s_prev = s;
-          if (++s == kStages) { s = 0; ph ^= 1; }
-        }
-        wgmma_wait<0>();
-        wgmma_reg_fence(acc);
+        if (p.ab8) mma_loop(std::true_type{});
+        else mma_loop(std::false_type{});
       }
-    };
-    // Block-scaled A: each 128-byte e4m3 k-block holds two 64-element units with their own row scales.  A unit's two
-    // k32 wgmmas go to a fresh partial that is promoted as acc = fma(part, s_a[row], acc).  The thread's fragment rows
-    // are r and r + 8 (acc[i] belongs to row r + 8 ((i / 2) % 2)); their scales are loaded before the stage's wait,
-    // and only for rows that exist (TMA zero-fills A past the matrix or the utterance, a plain load would not).
-    auto mma_loop_scaled = [&]() {
-      const uint32_t ring = smem_u32(smem);
-      int s = 0;
-      uint32_t ph = 0;
-      const int t0 = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
-      const int lim = p.tiles_per_batch > 0 ? p.rows_per_batch - m_in_batch0 : p.M - row0;   // rows of the tile that exist
-      const bool ok0 = t0 < lim, ok1 = t0 + 8 < lim;
-      const float* sp = p.a_scale + row0 + t0;
-      const size_t ld = (size_t)p.a_scale_ld;
-      float part[BN / 2];
-      for (int kb = 0; kb < num_kb; ++kb) {
-        float sc[2][2];   // [unit][row]
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const float* su = sp + (size_t)(2 * kb + u) * ld;
-          sc[u][0] = ok0 ? su[0] : 0.f;
-          sc[u][1] = ok1 ? su[8] : 0.f;
-        }
-        mbar_wait(&full_bar[s], ph);
-        const uint32_t sa = ring + s * S::kStageBytes + wg * (64 * 128), sb = ring + s * S::kStageBytes + S::kABytes;
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            gemm_wgmma<BN, true>(part, gmma_desc_sw128(sa + 64 * u + 32 * k, 16, 1024),
-                                 gmma_desc_sw128(sb + 64 * u + 32 * k, 16, 1024), k != 0);
-          wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_reg_fence(part);
-          if (u == 1) mbar_arrive(&empty_bar[s]);
-#pragma unroll
-          for (int i = 0; i < BN / 2; ++i) acc[i] = fmaf(part[i], sc[u][(i >> 1) & 1], acc[i]);
-        }
-        if (++s == kStages) { s = 0; ph ^= 1; }
-      }
-    };
-    if constexpr (SCALED) {
-      if (p.ab8 && p.a_scale != nullptr) mma_loop_scaled();
-      else if (p.ab8) mma_loop(std::true_type{});
-      else mma_loop(std::false_type{});
-    } else {
-      if (p.ab8) mma_loop(std::true_type{});
-      else mma_loop(std::false_type{});
-    }
+      mbar_arrive(mma_turn);
+      // PDL: the CTA's last main loop is done — let the next kernel of the stream start its prologue under this
+      // epilogue; it still waits (pdl_wait) for this grid to complete before touching memory
+      if (t + (int)gridDim.x >= gemm_tiles(p, BN)) pdl_launch_dependents();
 
-    // accumulator fragments -> fp32 tile in shared memory (row-major, kAccLd floats per row)
-    {
-      const int r = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
-      const int c = 2 * (lane & 3);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(acc_s + r * S::kAccLd + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(acc_s + (r + 8) * S::kAccLd + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
-    }
-    asm volatile("bar.sync 3, 256;" ::: "memory");   // accumulator tile and staged columns visible to both groups
-    // PDL: the main loop is done — let the next kernel of the stream start its prologue under this epilogue; it
-    // still waits (pdl_wait) for this grid to complete before touching memory
-    pdl_launch_dependents();
-    if (grp < E::kGroups) {
       // ===================== epilogue =====================
-      const int r_in_tile = et;
-      const int m_in_batch = m_in_batch0 + r_in_tile;
-      const int row = row0 + r_in_tile;
+      const GemmTile g = gemm_tile(p, t, BN);   // (not held in registers across the main loop)
+      if (!first) mbar_wait(epi_free, turn_par);   // tile j - 1's epilogue is done with the shared tile
+      // accumulator fragments -> the fp32 boxes (SWIZZLE_128B: 16-byte piece q of row r at (q ^ (r & 7)) * 16)
+      {
+        const int sw = wr & 7;   // = (wr + 8) & 7 = (wr + 64) & 7
+        uint8_t* base = acc_tile + wr * 128 + (lane & 1) * 8;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int q = 0; q < BN / 8; ++q) {   // columns 8 q + 2 (lane % 4) + {0, 1}
+            uint8_t* pc = base + h * (64 * 128) + (q >> 2) * 16384 + (((2 * (q & 3) + ((lane >> 1) & 1)) ^ sw) << 4);
+            *reinterpret_cast<float2*>(pc) = make_float2(acc[h][4 * q], acc[h][4 * q + 1]);
+            *reinterpret_cast<float2*>(pc + 8 * 128) = make_float2(acc[h][4 * q + 2], acc[h][4 * q + 3]);
+          }
+      }
+      epi_stage_cols<BN, SCALED>(p, g.n0, et, bias_s, gate_s, aux_s, ws_s);
+      const int m_in_batch = g.m_in_batch0 + et;
+      const int row = g.row0 + et;
       bool row_ok;
       int b_idx, pos;
       if (p.tiles_per_batch > 0) {
         row_ok = m_in_batch < p.rows_per_batch;
-        b_idx = batch;
+        b_idx = g.batch;
         pos = m_in_batch;
       } else {
         row_ok = row < p.M;
@@ -314,25 +369,26 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
       float2 cs[ROPE ? 32 : 1];
       epi_load_rope<ROPE>(p, pos, cs);
       float4 res0[8];
-      epi_load_resid(p, row, n0g, row_ok, res0);
-      // every MMA has retired, so the operand ring is idle: its first 32 KB per group stage the stores
+      if constexpr (!(ROPE || SCALED)) epi_load_resid(p, row, g.n0, row_ok, res0);   // else in epi_drain_tile
       EpiStage stg;
-      stg.buf = smem + grp * 32768;
+      stg.acc = acc_tile;
+      stg.stg = smem + S::kStgOffset;
       stg.et = et;
-      stg.r = r_in_tile;
+      stg.r = et;
       stg.map_out = &tma_out;
       stg.map_out2 = &tma_out2;
-      stg.c1 = m_in_batch0;
-      stg.c2 = p.tiles_per_batch > 0 ? batch : 0;
-      stg.bar_id = 1 + grp;
-      stg.buf2 = smem + 65536 + grp * 16384;
-      stg.buf2_par = 8192;
+      stg.c1 = g.m_in_batch0;
+      stg.c2 = g.batch;
+      stg.bar_id = 1 + wg;
       stg.mu_r = ln_mu_r; stg.rstd = ln_rstd;
       stg.out_fp8 = p.out_fp8;
-      epi_drain_tile<BNG, ACT, OUT_BF16, ROPE, SCALED>(acc_s + r_in_tile * S::kAccLd + grp * BNG, bias_s, gate_s, aux_s,
-                                                       cs, res0, p, n0g, row, row_ok, row_valid, stg, ws_s);
-      if (et == 0) tma_store_wait_read<0>();   // the staging buffers must outlive the TMA unit's reads; grid completion
-                                               // makes the global writes visible to the dependent kernel
+      asm volatile("bar.sync %0, 128;" ::"r"(stg.bar_id) : "memory");   // accumulator tile and staged columns visible
+      epi_drain_tile<BN, ACT, OUT_BF16, ROPE, SCALED>(bias_s, gate_s, aux_s, cs, res0, p, g.n0, row, row_ok, row_valid,
+                                                      stg, ws_s);
+      // the next tile may rewrite the accumulator tile and the staging once the TMA unit has read them; grid
+      // completion makes the global writes visible to the dependent kernel
+      if (et == 0) tma_store_wait_read<0>();
+      mbar_arrive(epi_free);
     }
   }
 
