@@ -6,7 +6,7 @@ does not need a GPU; every compute call does (there is no CPU fallback).
 """
 from .weights import BASE_CONFIG, GATE_CONFIG, DiTConfig, VocosConfig  # noqa: F401
 from .dit import DiT  # noqa: F401
-from .audio import MelSpec, log_mel_spectrogram  # noqa: F401
+from .audio import MelSpec, log_mel_spectrogram, resample  # noqa: F401
 from .cfm import CFM, F5TTS, odeint_euler, odeint_midpoint, odeint_rk4  # noqa: F401
 
 __version__ = "0.1.0"

@@ -135,6 +135,9 @@ SYMBOLS: dict[str, tuple] = {
     "f5_duration_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_mel_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                  C.c_void_p, C.c_int32, C.c_void_p]),
+    "f5_resample_table": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int64]),
+    "f5_resample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                              C.c_int64, C.c_void_p]),
     "f5_istft": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                            C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "f5_vocos_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

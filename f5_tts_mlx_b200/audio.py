@@ -2,7 +2,8 @@
 
 The arithmetic (zero-padded centred framing, periodic-Hann 1024-point real FFT, magnitude, HTK mel
 filterbank, log(max(., 1e-5))) runs in the sm_90a kernel behind `f5_mel_forward`; this module only
-builds the two constant tables (window, filterbank) and marshals pointers.
+builds the two constant tables (window, filterbank) and marshals pointers.  `resample` converts other sample
+rates to and from the model's 24 kHz in the kernel behind `f5_resample`.
 """
 from __future__ import annotations
 
@@ -68,6 +69,47 @@ def log_mel_spectrogram(audio: torch.Tensor, sample_rate: int = 24_000, n_mels: 
             n_mels, hop_length, C.c_void_p(out.data_ptr()), frames,
             C.c_void_p(torch.cuda.current_stream().cuda_stream)))
     return out
+
+
+@lru_cache(maxsize=16)
+def _resample_table(orig_freq: int, new_freq: int, device: str) -> torch.Tensor:
+    # the filter is defined once, in f5_resample_table (include/f5_b200.h); this only uploads it
+    lib = _lib.load()
+    n = lib.f5_resample_table(orig_freq, new_freq, None, 0)
+    if n < 0:
+        _lib.check(n)
+    host = torch.empty(max(n, 1), dtype=torch.float32)
+    rc = lib.f5_resample_table(orig_freq, new_freq, C.cast(host.data_ptr(), C.POINTER(C.c_float)), n)
+    if rc < 0:
+        _lib.check(rc)
+    return host.to(device)
+
+
+def resample(wave: torch.Tensor, orig_freq: int, new_freq: int) -> torch.Tensor:
+    """torchaudio.functional.resample at its defaults (the windowed-sinc filter upstream F5-TTS resamples reference
+    clips with), in the sm_90a kernel behind `f5_resample`: CUDA fp32 [t] or [b, t] at orig_freq -> the same rank at
+    new_freq, ceil(t * new / orig) samples.  Equal rates return `wave` itself."""
+    orig_freq, new_freq = int(orig_freq), int(new_freq)
+    if orig_freq <= 0 or new_freq <= 0:
+        raise ValueError(f"sample rates must be positive, got {orig_freq} -> {new_freq}")
+    if not wave.is_cuda:
+        raise _lib.F5Error("resample needs a CUDA tensor: there is no CPU path")
+    if wave.ndim not in (1, 2):
+        raise ValueError(f"resample takes [t] or [b, t], got shape {tuple(wave.shape)}")
+    if orig_freq == new_freq:
+        return wave
+    x = wave.float().contiguous()
+    x2 = x[None] if x.ndim == 1 else x
+    b, t = x2.shape
+    g = math.gcd(orig_freq, new_freq)
+    out_len = -(-(new_freq // g) * t // (orig_freq // g))
+    out = torch.empty(b, out_len, device=x.device, dtype=torch.float32)
+    if b > 0 and t > 0:
+        table = _resample_table(orig_freq, new_freq, str(x.device))
+        _lib.check(_lib.load().f5_resample(
+            C.c_void_p(x2.data_ptr()), b, t, orig_freq, new_freq, C.c_void_p(table.data_ptr()),
+            C.c_void_p(out.data_ptr()), out_len, C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    return out[0] if wave.ndim == 1 else out
 
 
 class MelSpec:

@@ -16,7 +16,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .audio import MelSpec
+from .audio import MelSpec, resample
 from .dit import DiT, DitSession, _check_prefix_padding
 from .utils import default, exists, lens_to_mask, list_str_to_idx, list_str_to_tensor, pad_sequence
 
@@ -230,6 +230,7 @@ class F5TTS:
         return_trajectory: bool = True,
         pad_frames: Optional[int] = None,
         frame_bucket: Optional[int] = None,
+        cond_sample_rate: Optional[int] = None,
     ) -> Tuple[torch.Tensor, torch.Tensor]:
         """cfm.py:264-402.  Extensions (default-compatible): `y0` injects the initial noise
         (b, n, mel) — MLX's RNG stream cannot be reproduced, so seeded parity is defined on injected
@@ -237,17 +238,27 @@ class F5TTS:
         final state with a leading axis of 1); `pad_frames` pads the batch to at least that many frames — a shard
         of a ragged batch must use the GLOBAL maximum (parallel.global_frames) to reproduce the unsharded result,
         because the reference's padding leaks into GRN and the ODE on padded frames; `frame_bucket` (default
-        self.frame_bucket) reuses one plan / CUDA graph for all lengths of a bucket, results unchanged."""
+        self.frame_bucket) reuses one plan / CUDA graph for all lengths of a bucket, results unchanged;
+        `cond_sample_rate` is the rate of a raw-wave `cond` (None: the mel front-end's own rate, 24 kHz) — another rate
+        is resampled on the device (audio.resample, torchaudio's default windowed sinc) before the mel."""
         dev = self.transformer.device
         if method not in METHODS:
             raise ValueError(f"Unknown method: {method}")
 
         # raw wave (cfm.py:283-286)
+        resample_from = None
+        if cond_sample_rate is not None and int(cond_sample_rate) != self._mel_spec.sample_rate:
+            resample_from = int(cond_sample_rate)
         if cond.ndim == 2:
             if cond.shape[0] != 1:
                 raise ValueError("raw-wave conditioning must have batch 1 (cfm.py:284)")
-            cond = self._mel_spec(cond[0].to(dev))
+            wave = cond[0].to(dev)
+            if resample_from is not None:
+                wave = resample(wave, resample_from, self._mel_spec.sample_rate)
+            cond = self._mel_spec(wave)
             assert cond.shape[-1] == self.num_channels
+        elif resample_from is not None:
+            raise ValueError("cond_sample_rate applies to a raw-wave cond [1, t]; this cond is a mel spectrogram")
         cond = cond.to(dev).float()
         batch, cond_seq_len = cond.shape[:2]
         if not exists(lens):

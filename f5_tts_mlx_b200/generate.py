@@ -1,12 +1,12 @@
 """generate() — host-side mirror of f5_tts_mlx/generate.py:113-244 (+ a real `main()`, which the
 reference's console script points at but never defines).
 
-Same keyword arguments and flow: load the 24 kHz reference clip, RMS-normalise it to 0.1 if quieter,
-split the text into sentences, one `F5TTS.sample()` per sentence with the SAME reference audio,
-strip the reference samples from each waveform, concatenate, write a wav.  Deviations: wav I/O uses
-the stdlib `wave` module (soundfile is not in the image); live playback (AudioPlayer, sounddevice)
-is out of scope, so `output_path=None` just returns the waveform; `duration=None` without
-`estimate_duration` needs a duration predictor exactly like the reference (ValueError otherwise).
+Same keyword arguments and flow: load the 24 kHz reference clip (any rate with `resample_ref_audio`),
+RMS-normalise it to 0.1 if quieter, split the text into sentences, one `F5TTS.sample()` per sentence with
+the SAME reference audio, strip the reference samples from each waveform, concatenate, write a wav.
+Deviations: wav files are read by a small RIFF chunk reader and written by the stdlib `wave` module
+(soundfile is not in the image); live playback (AudioPlayer, sounddevice) is out of scope, so
+`output_path=None` just returns the waveform; `duration=None` without `estimate_duration` needs a duration predictor exactly like the reference (ValueError otherwise).
 
 Pinned against the reference's own generate() executed through tests/mlx_shim
 (tests/golden/ref_generate_calls.json, tests/test_ref_pins.py): sentence split, text assembly,
@@ -22,12 +22,14 @@ from __future__ import annotations
 import argparse
 import datetime
 import re
+import struct
 import wave as wavmod
 from typing import Literal, Optional
 
 import numpy as np
 import torch
 
+from .audio import resample
 from .cfm import F5TTS
 from .utils import convert_char_to_pinyin
 
@@ -57,13 +59,54 @@ def estimated_duration(ref_audio: torch.Tensor, ref_text: str, gen_text: str, sp
     return duration_in_frames / FRAMES_PER_SEC
 
 
+WAVE_FORMAT_PCM, WAVE_FORMAT_IEEE_FLOAT, WAVE_FORMAT_EXTENSIBLE = 0x0001, 0x0003, 0xFFFE
+
+
+def _wav_chunks(raw: bytes, path: str):
+    """RIFF/WAVE chunk reader: {chunk id: payload} of the top-level chunks (first occurrence of each)."""
+    if len(raw) < 12 or raw[:4] != b"RIFF" or raw[8:12] != b"WAVE":
+        raise ValueError(f"{path}: not a RIFF/WAVE file")
+    chunks, pos = {}, 12
+    while pos + 8 <= len(raw):
+        cid, size = raw[pos:pos + 4], struct.unpack_from("<I", raw, pos + 4)[0]
+        chunks.setdefault(cid, raw[pos + 8:pos + 8 + size])       # a truncated last chunk keeps what is there
+        pos += 8 + size + (size & 1)                               # chunks are padded to an even size
+    return chunks
+
+
 def read_wav(path: str):
-    with wavmod.open(path, "rb") as f:
-        sr, ch, sw, n = f.getframerate(), f.getnchannels(), f.getsampwidth(), f.getnframes()
-        raw = f.readframes(n)
-    if sw != 2:
-        raise ValueError("only 16-bit PCM wav files are supported")
-    x = np.frombuffer(raw, dtype=np.int16).astype(np.float32) / 32768.0
+    """Mono fp32 waveform and sample rate of a WAV file: 8-bit unsigned, 16-, 24- and 32-bit PCM, or 32-bit IEEE
+    float, with a plain or WAVE_FORMAT_EXTENSIBLE header; channels are averaged.  Integer PCM is scaled by 2^-(bits-1)
+    (16-bit: x / 32768), float samples are taken as they are.  Other formats raise ValueError."""
+    with open(path, "rb") as f:
+        chunks = _wav_chunks(f.read(), path)
+    fmt, data = chunks.get(b"fmt "), chunks.get(b"data")
+    if fmt is None or len(fmt) < 16 or data is None:
+        raise ValueError(f"{path}: WAVE file without a complete 'fmt ' and 'data' chunk")
+    tag, ch, sr, _, block, bits = struct.unpack_from("<HHIIHH", fmt)
+    if tag == WAVE_FORMAT_EXTENSIBLE:
+        if len(fmt) < 40:
+            raise ValueError(f"{path}: WAVE_FORMAT_EXTENSIBLE header of {len(fmt)} bytes (< 40)")
+        tag = struct.unpack_from("<H", fmt, 24)[0]                 # first two bytes of the SubFormat GUID
+    kind = {(WAVE_FORMAT_PCM, 8): "u8", (WAVE_FORMAT_PCM, 16): "s16", (WAVE_FORMAT_PCM, 24): "s24",
+            (WAVE_FORMAT_PCM, 32): "s32", (WAVE_FORMAT_IEEE_FLOAT, 32): "f32"}.get((tag, bits))
+    if kind is None or ch < 1 or block != ch * bits // 8:
+        name = {WAVE_FORMAT_PCM: "PCM", WAVE_FORMAT_IEEE_FLOAT: "IEEE float"}.get(tag, f"format tag 0x{tag:04x}")
+        raise ValueError(f"{path}: unsupported WAV format: {name}, {bits} bits, {ch} channel(s); supported are "
+                         "8-bit unsigned, 16-, 24- and 32-bit PCM and 32-bit IEEE float")
+    raw = data[: len(data) // block * block]
+    if kind == "s16":
+        x = np.frombuffer(raw, dtype="<i2").astype(np.float32) / 32768.0
+    elif kind == "u8":
+        x = (np.frombuffer(raw, dtype=np.uint8).astype(np.float32) - 128.0) / 128.0
+    elif kind == "s24":
+        b3 = np.frombuffer(raw, dtype=np.uint8).reshape(-1, 3).astype(np.int32)
+        v = b3[:, 0] | (b3[:, 1] << 8) | (b3[:, 2] << 16)
+        x = (v - ((v & 0x800000) << 1)).astype(np.float32) / 8388608.0
+    elif kind == "s32":
+        x = (np.frombuffer(raw, dtype="<i4").astype(np.float64) / 2147483648.0).astype(np.float32)
+    else:
+        x = np.frombuffer(raw, dtype="<f4").astype(np.float32)
     if ch > 1:
         x = x.reshape(-1, ch).mean(axis=1)
     return torch.from_numpy(x), sr
@@ -96,6 +139,8 @@ def generate(
     frame_bucket: int = 128,
     fp8: Optional[str] = None,
     fp8_attention: bool = False,
+    resample_ref_audio: bool = False,
+    output_sample_rate: int = SAMPLE_RATE,
 ):
     """generate.py:113-244.  Extensions: `f5tts` reuses a loaded model; `batch_sentences=True` runs all
     sentences as ONE ragged `sample()` batch instead of the reference's serial loop
@@ -104,9 +149,15 @@ def generate(
     the sentences of the serial loop share one set of buffers and ONE captured CUDA graph per length bucket instead of
     re-capturing for every distinct length (0 = the exact shapes); results are unchanged (F5TTS.sample).  `fp8`: None
     (bf16), "tensor" or "block" — the lossy FP8 mode of the DiT and its scaling (DESIGN.md section 8);
-    `fp8_attention` (with fp8="block"): the attention on e4m3 Q, K and V as well."""
+    `fp8_attention` (with fp8="block"): the attention on e4m3 Q, K and V as well.  `resample_ref_audio`: a reference
+    clip at any sample rate is RMS-normalised, then resampled to 24 kHz on the GPU (audio.resample, torchaudio's
+    default windowed sinc, as upstream F5-TTS does); without it a clip that is not 24 kHz is refused, as in the
+    reference.  `output_sample_rate`: the returned / written waveform is resampled from 24 kHz to this rate."""
     if fp8_attention and fp8 != "block":
         raise ValueError('fp8_attention needs fp8="block"')
+    output_sample_rate = int(output_sample_rate)
+    if output_sample_rate <= 0:
+        raise ValueError(f"output_sample_rate must be positive, got {output_sample_rate}")
     if f5tts is None:
         f5tts = F5TTS.from_pretrained(model_name, quantization_bits=quantization_bits, fp8=fp8,
                                       fp8_attention=fp8_attention)
@@ -117,15 +168,19 @@ def generate(
     if ref_audio_path is None:
         raise ValueError("ref_audio_path is required (the reference's packaged default clip is not redistributed here)")
     audio, sr = read_wav(ref_audio_path)
-    if sr != SAMPLE_RATE:
-        raise ValueError("Reference audio must have a sample rate of 24kHz")      # generate.py:147-148
+    if sr != SAMPLE_RATE and not resample_ref_audio:                              # generate.py:147-148
+        raise ValueError(f"Reference audio must have a sample rate of 24kHz (got {sr} Hz; "
+                         "resample_ref_audio=True / --resample converts it)")
     if ref_audio_text is None:
         ref_audio_text = DEFAULT_REF_TEXT
-    print(f"Got reference audio with duration: {audio.shape[0] / SAMPLE_RATE:.2f} seconds")
+    print(f"Got reference audio with duration: {audio.shape[0] / sr:.2f} seconds")
     rms = torch.sqrt(torch.mean(torch.square(audio)))
     if rms < TARGET_RMS:
         audio = audio * TARGET_RMS / rms                                          # generate.py:154-156
     audio_d = audio.to(dev)
+    if sr != SAMPLE_RATE:
+        audio_d = resample(audio_d, sr, SAMPLE_RATE)                              # normalised first, as upstream
+    ref_len = audio_d.shape[0]                                                    # reference samples at 24 kHz
 
     sentences = split_sentences(generation_text)
     single = len(sentences) <= 1 or duration is not None                          # generate.py:158-159
@@ -141,7 +196,7 @@ def generate(
         mel = f5tts._mel_spec(audio_d)                                    # (1, n_ref, 100), computed once
         texts = convert_char_to_pinyin([ref_audio_text + " " + s_ for s_ in todo])
         if duration is None and estimate_duration:
-            durs = torch.tensor([int(estimated_duration(audio, ref_audio_text, s_, speed) * FRAMES_PER_SEC) for s_ in todo])
+            durs = torch.tensor([int(estimated_duration(audio_d, ref_audio_text, s_, speed) * FRAMES_PER_SEC) for s_ in todo])
         elif duration is None:
             durs = None
         else:
@@ -158,23 +213,25 @@ def generate(
         lens_i = plan.session.seq_len[: len(todo)].tolist() if plan.session.seq_len is not None else [out.shape[1]] * len(todo)
         for i in range(len(todo)):
             wave_i = vocoder(out[i:i + 1, : lens_i[i]]) if vocoder is not None else out[i, : lens_i[i]]
-            waves.append(wave_i[audio.shape[0]:] if vocoder is not None else wave_i)
+            waves.append(wave_i[ref_len:] if vocoder is not None else wave_i)
         todo = []
     for sentence in todo:
         if duration is None and estimate_duration:
-            frames = int(estimated_duration(audio, ref_audio_text, sentence if not single else generation_text, speed)
+            frames = int(estimated_duration(audio_d, ref_audio_text, sentence if not single else generation_text, speed)
                          * FRAMES_PER_SEC)
         text = convert_char_to_pinyin([ref_audio_text + " " + sentence])
         wave, _ = f5tts.sample(audio_d[None], text=text, duration=frames, steps=steps, method=method, speed=speed,
                                cfg_strength=cfg_strength, sway_sampling_coef=sway_sampling_coef, seed=seed,
                                return_trajectory=False, frame_bucket=frame_bucket)
-        waves.append(wave[audio.shape[0]:])                                       # strip the reference (generate.py:183)
+        waves.append(wave[ref_len:])                                              # strip the reference (generate.py:183)
     wave = torch.cat(waves, dim=0)
     if wave.is_cuda:
         torch.cuda.synchronize()
     print(f"Generated {wave.shape[0] / SAMPLE_RATE:.2f}s of audio in {datetime.datetime.now() - start}.")
+    if output_sample_rate != SAMPLE_RATE:
+        wave = resample(wave, SAMPLE_RATE, output_sample_rate)
     if output_path is not None:
-        write_wav(output_path, wave)
+        write_wav(output_path, wave, output_sample_rate)
     return wave
 
 
@@ -198,6 +255,10 @@ def main(argv=None) -> None:
                    help="run the DiT's GEMMs on e4m3 operands (lossy) with per-tensor or block (per-channel / per-64) scales")
     p.add_argument("--fp8-attention", action="store_true",
                    help="with --fp8 block: run the attention's Q·K^T and P·V on e4m3 too (lossy)")
+    p.add_argument("--resample", action="store_true",
+                   help="accept a reference clip at any sample rate: resample it to 24 kHz on the GPU")
+    p.add_argument("--output-sample-rate", type=int, default=SAMPLE_RATE,
+                   help="sample rate of the written waveform (resampled on the GPU from 24 kHz)")
     a = p.parse_args(argv)
     if a.fp8_attention and a.fp8 != "block":
         p.error("--fp8-attention needs --fp8 block")
@@ -210,7 +271,8 @@ def main(argv=None) -> None:
     generate(generation_text=a.text, duration=a.duration, estimate_duration=a.estimate_duration, model_name=a.model,
              ref_audio_path=a.ref_audio, ref_audio_text=a.ref_text, steps=a.steps, method=a.method, cfg_strength=a.cfg,
              sway_sampling_coef=a.sway_coef, speed=a.speed, seed=a.seed, quantization_bits=a.q, output_path=a.output,
-             fp8=a.fp8, fp8_attention=a.fp8_attention)
+             fp8=a.fp8, fp8_attention=a.fp8_attention, resample_ref_audio=a.resample,
+             output_sample_rate=a.output_sample_rate)
 
 
 if __name__ == "__main__":

@@ -433,6 +433,32 @@ int f5_mel_forward(const float* audio, int32_t batch, int32_t samples, const flo
                    void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
+ * Sample-rate conversion (ABI 2.003) — torchaudio.functional.resample at its defaults (sinc_interp_hann,
+ * lowpass_filter_width 6, rolloff 0.99), the resampler upstream F5-TTS puts in front of the mel front-end for
+ * reference clips that are not 24 kHz.  With g = gcd(orig, new), O = orig / g, N = new / g:
+ *
+ *     base = min(O, N) * 0.99;   w = ceil(6 * O / base);   taps = 2 * w + O
+ *     for phase p in [0, N), tap k in [0, taps):
+ *         t = clamp(((k - w) / O - p / N) * base, -6, 6)
+ *         h[p][k] = (t == 0 ? 1 : sin(pi t) / (pi t)) * cos(pi t / 12)^2 * base / O
+ *     out_samples = ceil(N * samples / O)
+ *     y[j] = sum_{k ascending} h[j % N][k] * x[(j / N) * O + k - w]        (x = 0 outside [0, samples))
+ *
+ * f5_resample_table : HOST function: returns N * taps, and writes h row-major [N][taps] to h_table when h_table is
+ *                     non-NULL and cap >= N * taps (computed in double, rounded once to fp32).  orig == new is the
+ *                     identity and returns 0.  F5_ERR_INVALID for a non-positive rate or a table of more than 65536
+ *                     entries (every pair of 8, 11.025, 16, 22.05, 32, 44.1, 48, 88.2, 96 kHz with 24 kHz fits).
+ * f5_resample       : x fp32 [batch, samples] -> out fp32 [batch, out_samples] with the table above (device memory);
+ *                     out_samples must equal ceil(N * samples / O).  Each output is one fp32 fused multiply-add chain
+ *                     in ascending k: bitwise reproducible, rows independent.  orig == new copies x to out (table
+ *                     may be NULL).  F5_ERR_INVALID also when one tile's input window exceeds shared memory
+ *                     (decimation by more than about 200:1).  x and out 4-byte aligned.
+ * ------------------------------------------------------------------------------------------ */
+int f5_resample_table(int32_t orig_freq, int32_t new_freq, float* h_table, int64_t cap);
+int f5_resample(const float* x, int32_t batch, int64_t samples, int32_t orig_freq, int32_t new_freq,
+                const float* table, float* out, int64_t out_samples, void* stream);
+
+/* ------------------------------------------------------------------------------------------ *
  * Vocos vocoder — replaces vocos_mlx.Vocos.decode (third-party; call sites cfm.py:399-400,446,
  * 471): Conv1d(100->512,k7) LN 8x[dwconv7 LN Linear GELU Linear gamma* +res] LN Linear(512->1026)
  * -> (log-mag, phase) -> ISTFT(n_fft 1024, hop 256).
