@@ -48,13 +48,53 @@ def round_to(ref: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
 
 
 def instantiation(*, act: int = 0, out_dtype=torch.bfloat16, rope: bool = False, fp8: bool = False,
-                  resid: bool = False, tile: int, conv_grouped: bool = False) -> tuple:
-    """(ACT, OUT_BF16, ROPE, FP8, RESID, BN) of the gemm_bf16_tn_kernel a launch selects (dispatch_epi in gemm.cu):
-    FP8 when any operand or output is e4m3, RESID = false only for the residual-free GELU-tanh bf16 epilogue, and
-    the grouped convolution always runs 64-column tiles."""
+                  resid: bool = False, tile: int, conv_grouped: bool = False, scaled: bool = False) -> tuple:
+    """(ACT, OUT_BF16, ROPE, FP8, RESID, BN) of the gemm_bf16_tn_kernel a launch selects.  dispatch_epi (gemm.cu): FP8
+    when any operand or output is e4m3, RESID = false only for the residual-free GELU-tanh bf16 epilogue.
+    dispatch_scaled (`scaled`: any block scale is set): always FP8, and its bf16-output forms (the RoPE QKV, FF1) carry
+    no residual.  The grouped convolution always runs 64-column tiles.  The SCALED template flag is `scaled` itself:
+    a scaled and an unscaled launch may share the other five flags and still run different kernels."""
     out_bf16 = out_dtype != torch.float32
+    if scaled:
+        return (act, out_bf16, rope, True, not out_bf16, 64 if conv_grouped else tile)
     no_resid = not resid and act == 1 and out_bf16 and not rope
     return (act, out_bf16, rope, fp8, not no_resid, 64 if conv_grouped else tile)
+
+
+# ---------------------------------------------------------------- launch geometry (gemm.cu f5_gemm_bf16)
+STAGES = {64: 6, 128: 4}     # ring depth of the 64- and 128-wide instantiations (dispatch_* <BN, kStages>)
+
+
+def cdiv(a: int, b: int) -> int:
+    return -(-a // b)
+
+
+def gemm_bn(n: int, m: int, *, tile_n: int = 0, rows_per_batch: int = 0, num_batches: int = 1, batched: bool = False,
+            conv_grouped: bool = False, sms: int) -> int:
+    """The launcher's tile width: tile_n when given, 64 for the grouped convolution, else 128 unless that leaves most
+    of the SMs idle (fewer than 13/16 of them get a tile) or n <= 64."""
+    if conv_grouped:
+        return 64
+    if tile_n:
+        return tile_n
+    rpb = rows_per_batch or m
+    mt = num_batches * cdiv(rpb, 128) if batched else cdiv(m, 128)
+    if n <= 64:
+        return 64
+    return 128 if mt * cdiv(n, 128) >= (sms * 13) // 16 else 64
+
+
+def gemm_tile_count(n: int, m: int, bn: int, *, rows_per_batch: int = 0, num_batches: int = 1,
+                    batched: bool = False) -> int:
+    """Output tiles of a launch: 128-row tiles over the flat rows, or over each utterance when tiles never straddle
+    utterances (batched / conv mode), times the column tiles.  The persistent grid is min(tiles, SMs) CTAs."""
+    rpb = rows_per_batch or m
+    return cdiv(n, bn) * (num_batches * cdiv(rpb, 128) if batched else cdiv(m, 128))
+
+
+def gemm_num_kb(k: int, *, conv_taps: int = 1, ab8: bool = False) -> int:
+    """k-blocks per tile (128 bytes of every row: 64 bf16 or 128 e4m3 elements, per tap)."""
+    return conv_taps * cdiv(k, 128 if ab8 else 64)
 
 
 # ---------------------------------------------------------------- tile naming

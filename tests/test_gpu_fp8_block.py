@@ -142,8 +142,7 @@ def test_scaled_gelu_e4m3_output(tile):
     go.check("gelu out guard"); so.check("gelu scale guard")
 
 
-# the RoPE QKV: bf16 out and no residual (instantiation() assumes a residual tile for every non-GELU epilogue)
-INSTANTIATIONS += [(0, True, True, True, False, 64), (0, True, True, True, False, 128)]
+_declare(rope=True, scaled=True)                     # the RoPE QKV: bf16 out, no residual
 
 
 @pytest.mark.parametrize("tile", [64, 128])

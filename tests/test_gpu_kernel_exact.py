@@ -6,15 +6,19 @@ then an integer (or a dyadic fraction with few bits) below 2^20, so the fp32 res
 fp32 outputs must equal the float64 reference bitwise, bf16 / e4m3 outputs its round-to-nearest, ln_stats exactly.
 Any indexing, masking, tail or ring-phase mistake is a nonzero difference, reported with its tile, row and column.
 Every output is written into a NaN-filled buffer with guard rows and columns (ld > n), which must stay untouched.
+Block-scaled operands carry power-of-two scales, so they stay exact too; block-scaled e4m3 outputs must equal the scale
+rule of the float64 result bitwise.  After an activation (tanh.approx, __expf / __logf, erff) no exact answer exists:
+the output is checked against a float64 bound and bitwise against the same GEMM run in one-wave slices.
 
-INSTANTIATIONS lists the kernel instantiation (gemm.cu dispatch_epi) each GEMM case launches; a CPU test checks it
+INSTANTIATIONS lists the kernel instantiation (gemm.cu dispatch_epi) each GEMM case below launches; a CPU test checks it
 against gemm.cu so that no instantiation and tile width goes untested.
 """
 import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_check import Guarded, assert_exact, attn_tiles, gemm_tiles, instantiation, round_to, rope_ref
+from kernel_check import (E4M3_SUB, U32, U_E4M3, Guarded, act_bound, act_ref, assert_exact, assert_within, attn_tiles,
+                          cdiv, gemm_tile_count, gemm_tiles, instantiation, out_bound, round_to, rope_ref)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -53,38 +57,146 @@ def row_lens(nb, rpb):
     return torch.tensor([(0, rpb // 2 + 1 if rpb > 1 else 1, rpb)[b % 3] for b in range(nb)], dtype=torch.int32, device=DEV)
 
 
+def pow2_scales(shape, seed, lo, hi):
+    """Block scales 2^e, e uniform in [lo, hi] (test_gpu_fp8_block._pow2 on the device)."""
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    return torch.exp2(torch.randint(lo, hi + 1, shape, generator=g, device=DEV).float())
+
+
+def ln_row_stats(M, units, seed):
+    """Fused-LN consumer input: per row (sum, sum of squares) of every 64-column unit such that mean and rstd are powers
+    of two (mean 2, variance 2^20: rstd 2^-10; mean -4, variance 2^16: rstd 2^-8; the LayerNorm's 1e-6 is below half an
+    ulp of the variance).  The kernel divides the sums by 64 * units, exactly only when units is a power of two."""
+    assert units & (units - 1) == 0, "the fused-LN consumer is exact only for K / 64 a power of two"
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    kind = torch.rand(M, generator=g, device=DEV) < 0.5
+    mean = torch.where(kind, 2.0, -4.0).double()
+    var = torch.where(kind, 2.0 ** 20, 2.0 ** 16).double()
+    stats = torch.empty(M, units, 2, device=DEV)
+    stats[..., 0] = (mean * 64)[:, None].float()
+    stats[..., 1] = ((var + mean * mean) * 64)[:, None].float()
+    return stats, mean, var.rsqrt()
+
+
+def granularity(x):
+    """The largest power of two 2^-e <= 1 (e <= 30) of which every element of x is a multiple."""
+    for e in range(31):
+        y = x * 2.0 ** e
+        if torch.equal(y, y.round()):
+            return 2.0 ** -e
+    raise AssertionError("reference is not a dyadic fraction with few bits")
+
+
+def assert_fp32_exact(x, what):
+    assert torch.equal(x.float().double(), x), f"{what}: the float64 reference is not exact in fp32 (operands too large)"
+
+
+def conv_ref(A, W, *, M, N, K, rpb, nb, taps, pad, grouped):
+    """float64 Conv1d of the implicit-GEMM operands: A [nb rpb, channels] (channels = N grouped, else K), W [N, taps K]
+    with W[n, t K + c] the weight of input channel c (of the column's 64-channel group when grouped) at tap t."""
+    cin = N if grouped else K
+    x = A.view(nb, rpb, cin).transpose(1, 2)
+    wt = W.view(N, taps, K).permute(0, 2, 1)
+    y = F.conv1d(x, wt, padding=pad, groups=N // 64 if grouped else 1)
+    return y.transpose(1, 2).reshape(M, N)
+
+
+def _sm_count():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
 def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.0, rpb=0, nb=1, batched=False,
-              row_len=False, gate=None, resid=None, out2=None, ln_scale=False, rope=False, ab8=False, pad_cols=0):
+              row_len=False, gate=None, resid=None, out2=None, ln_scale=False, rope=False, ab8=False, pad_cols=0,
+              act=0, scaled=False, out_blocks=False, scale_exp=(-3, 3), a_scale_ld=0, ln_in=False, conv_taps=1,
+              conv_pad=0, conv_grouped=False):
     """One GEMM launch against its float64 reference.  out: 'bf16' | 'f32' | 'e4m3'; gate: None | 'shared' (one [N]
-    vector for every utterance);
-    resid: None | 'alias' (resid is out itself) | 'sep'; out2: None | 'bf16' | 'e4m3'."""
+    vector for every utterance); resid: None | 'alias' (resid is out itself) | 'sep'; out2: None | 'bf16' | 'e4m3'.
+
+    scaled: block-scaled FP8 (dispatch_scaled) — A and W e4m3 codes from {0, +-1, +-2}, a_scale one power of two per
+    (row, 64-column unit) in a [K/64][a_scale_ld] buffer (default ld M + 8, the columns beyond M NaN), w_scale one per
+    channel, exponents in scale_exp; e4m3 outputs are then block-scaled (out_scale / out2_scale), and their codes and
+    scales must equal weights.quantize_e4m3_blocks of the float64 result bitwise.  out_blocks: block-scaled e4m3
+    outputs of bf16 operands (the Mish producer of the block-scaled mode).
+    ln_in: fused-LN consumer with power-of-two row statistics (ln_row_stats) and an integer c1 / c2 table.
+    conv_taps / conv_pad / conv_grouped: implicit Conv1d over batched utterances (conv_ref); K is the k per tap.
+    act (1 GELU-tanh, 2 GELU-erf, 3 Mish): the pre-activation is exact; the output must be (a) within act_bound of the
+    float64 activation and (b) bitwise equal to the same GEMM launched in slices of at most SMs tiles, in which every tile
+    is the first and only tile of its CTA."""
     from f5_tts_mlx_b200 import ops
+    from f5_tts_mlx_b200.weights import quantize_e4m3_blocks
     odt = {"bf16": torch.bfloat16, "f32": torch.float32, "e4m3": torch.uint8}[out]
     rpb_e = rpb or M
+    ab8 = ab8 or scaled
+    conv = conv_taps > 1 or conv_grouped
+    assert not (conv and ab8) and (not conv or (rpb and batched)), "conv mode: bf16 operands, batched utterances"
+    kin = N if conv_grouped else K
     if ab8:
         A, W = ints((M, K), 2, seed, density, F8), ints((N, K), 2, seed + 1, density, F8)
-        acc_scale = 0.5
+        acc_scale = 1.0 if scaled else 0.5
     else:
-        A, W = ints((M, K), amax, seed, density), ints((N, K), amax, seed + 1, density)
+        A, W = ints((M, kin), amax, seed, density), ints((N, conv_taps * K), amax, seed + 1, density)
         acc_scale = 1.0
     bias = ints((N,), 8, seed + 2, dtype=torch.float32)
     rows = torch.arange(M, device=DEV)
     bidx, pos = rows // rpb_e, rows % rpb_e
     A64, W64 = A.float().double(), W.float().double()
-    v = (A64 @ W64.T) * acc_scale + bias.double()
-    vb = (A64.abs() @ W64.abs().T) * acc_scale + bias.double().abs()      # bounds every partial sum
     kw = dict(bias=bias, tile_n=tile, w_static=bool(w_static), ab_fp8=ab8, acc_scale=acc_scale)
+    colscale = torch.full((N,), acc_scale, dtype=torch.float64, device=DEV)
+    sa_buf = None
+    if scaled:
+        units = K // 64
+        sa_buf = torch.full((units, a_scale_ld or M + 8), float("nan"), device=DEV)
+        assert sa_buf.shape[1] >= M
+        sa = pow2_scales((units, M), seed + 7, *scale_exp)
+        sa_buf[:, :M] = sa
+        sw = pow2_scales((N,), seed + 8, *scale_exp)
+        A64 = (A64.view(M, units, 64) * sa.T.double()[..., None]).view(M, K)
+        colscale = sw.double()
+        kw.update(a_scale=sa_buf, w_scale=sw)
+    if conv:
+        cw = dict(M=M, N=N, K=K, rpb=rpb, nb=nb, taps=conv_taps, pad=conv_pad, grouped=conv_grouped)
+        acc, accb = conv_ref(A64, W64, **cw), conv_ref(A64.abs(), W64.abs(), **cw)
+        kw.update(n=N, k=K, conv_taps=conv_taps, conv_pad=conv_pad, conv_grouped=conv_grouped)
+    else:
+        acc, accb = A64 @ W64.T, A64.abs() @ W64.abs().T
+    assert (accb < EXACT_LIMIT).all(), "operands too large for an exact test"     # bounds every partial sum
+    stats = None
+    if ln_in:
+        stats, mean, rstd = ln_row_stats(M, K // 64, seed + 9)
+        tab = ints((4, N + 8), 8, seed + 10, dtype=torch.float32)            # ld > N
+        c1 = (tab[0] + tab[1])[:N].double()
+        c2 = (tab[2] + tab[3])[:N].double() + bias.double()
+        mu_r = (mean * rstd)[:, None]
+        v = rstd[:, None] * colscale[None] * acc - mu_r * c1[None] + c2[None]
+        vb = rstd[:, None] * colscale[None] * accb + (mu_r * c1[None]).abs() + c2.abs()[None]
+        kw.update(ln_in_stats=stats, ln_tab=tab)
+    else:
+        v = acc * colscale[None] + bias.double()
+        vb = accb * colscale[None] + bias.double().abs()
+    assert_fp32_exact(v, "pre-activation")
+    bnd = None                                     # None: v is exact; else |kernel - v| <= bnd before the output rounding
+    if act:
+        assert not rope
+        pre = v
+        v = act_ref(pre, act)
+        bnd = act_bound(pre, torch.zeros_like(pre), act)
+        kw.update(act=act)
     if rpb:
         kw.update(rows_per_batch=rpb, num_batches=nb, batched_tiles=batched)
     if rope:
-        tab = quarter_turns(rpb_e, seed + 3)
+        tab_r = quarter_turns(rpb_e, seed + 3)
         rc, qc = 2 * N // 3, N // 3
-        v = rope_ref(v, tab, pos, rc)
+        v = rope_ref(v, tab_r, pos, rc)
         v[:, :qc] *= 0.125
-        kw.update(rope=tab, rope_cols=rc, q_scale=0.125, q_cols=qc)
+        kw.update(rope=tab_r, rope_cols=rc, q_scale=0.125, q_cols=qc)
+    valid = torch.ones(M, dtype=torch.bool, device=DEV)
+    lens = None
     if row_len:
         lens = row_lens(nb, rpb_e)
-        v = torch.where((pos < lens.long()[bidx])[:, None], v, torch.zeros_like(v))
+        valid = pos < lens.long()[bidx]
+        v = torch.where(valid[:, None], v, torch.zeros_like(v))
+        if bnd is not None:
+            bnd = torch.where(valid[:, None], bnd, torch.zeros_like(bnd))
         kw.update(row_len=lens)
     g_out = Guarded(M, N, odt, DEV, pad_cols=pad_cols)
     if gate is not None:
@@ -92,7 +204,9 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
         gt = pow2((N,), seed + 4)
         gm = gt.double()[None]
         v, vb = v * gm, vb * gm.abs()
+        bnd = bnd * gm.abs() if bnd is not None else None
         kw.update(gate=gt)
+    r = None
     if resid is not None:
         r = ints((M, N), 16, seed + 5, dtype=torch.float32)
         v, vb = v + r.double(), vb + r.double().abs()
@@ -102,39 +216,172 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
             kw.update(resid=g_out.view)
         else:
             kw.update(resid=r)
-    assert (vb < EXACT_LIMIT).all(), "operands too large for an exact test"
-    g2 = st = None
+    if bnd is not None and (gate is not None or resid is not None):
+        bnd = bnd + U32 * v.abs()                  # v * gate + resid: one fma
+    if bnd is None:
+        assert (vb < EXACT_LIMIT).all(), "operands too large for an exact test"
+        assert_fp32_exact(v, "out")
+    blk_out, blk_out2 = (scaled or out_blocks) and out == "e4m3", (scaled or out_blocks) and out2 == "e4m3"
+    so = s2 = g2 = st = s = None
+    if blk_out:
+        so = Guarded(N // 64, M, torch.float32, DEV, lr=False)
+        kw.update(out_scale=so.view)
     if out2 is not None:
         g2 = Guarded(M, N, torch.uint8 if out2 == "e4m3" else torch.bfloat16, DEV)
         kw.update(out2=g2.view, out2_fp8=out2 == "e4m3")
+        if blk_out2:
+            s2 = Guarded(N // 64, M, torch.float32, DEV, lr=False)
+            kw.update(out2_scale=s2.view)
         if ln_scale:
             s = pow2((N,), seed + 6).abs() - 1          # 1 + s in {0.5, 1, 2}
             st = Guarded(M, N // 64 * 2, torch.float32, DEV, lr=False)
             kw.update(ln_scale=s, ln_stats=st.view.view(M, N // 64, 2))
             want2 = v * (1 + s.double())
-            assert (64 * vb.view(M, N // 64, 64).amax(-1) ** 2 < 2 ** 24).all(), "ln_stats would not be exact"
+            if bnd is None:   # every partial unit sum (of squares) is a multiple of gq (gq^2) below 2^24 of them
+                gq = granularity(v)
+                u = v.view(M, N // 64, 64) / gq
+                assert (u.abs().sum(-1) < 2 ** 24).all() and ((u * u).sum(-1) < 2 ** 24).all(), "ln_stats would not be exact"
         else:
             want2 = v
+        if out2 == "e4m3" and not blk_out2:
+            assert (want2.abs() + (bnd if bnd is not None else 0) * 2 < 448).all(), "per-tensor e4m3 out2 would saturate"
     ops.gemm(A, W, g_out.view, out_fp8=out == "e4m3", **kw)
     torch.cuda.synchronize()
-    loc = gemm_tiles(tile, rpb_e, batched)
+    loc = gemm_tiles(64 if conv_grouped else tile, rpb_e, batched)
     what = f"M={M} N={N} K={K} tile={tile} w_static={w_static}"
-    assert_exact(g_out.view, round_to(v, odt), loc, what + " out")
+    unit = lambda r_, c_: f"row {r_} unit {c_ // 2}"
+    if blk_out:
+        _check_blocks(g_out, so, v, bnd, loc, what + " out")
+    elif bnd is None:
+        assert_exact(g_out.view, round_to(v, odt), loc, what + " out")
+    else:
+        assert_within(g_out.view, v, out_bound(v, bnd, odt) + 1e-300, loc, what + " out")   # exact zeros: bound 0
     g_out.check(what + " out guard")
     if g2 is not None:
-        assert_exact(g2.view, round_to(want2, g2.view.dtype), loc, what + " out2")
+        sc = (1 + s.double()) if s is not None else torch.ones(N, dtype=torch.float64, device=DEV)
+        if blk_out2:
+            # the scale rule of the float64 result (exact), or of the kernel's own fp32 out when that is not exact
+            _check_blocks(g2, s2, want2 if bnd is None else g_out.view.double() * sc, None, loc, what + " out2")
+        elif bnd is None:
+            assert_exact(g2.view, round_to(want2, g2.view.dtype), loc, what + " out2")
+        else:
+            assert_within(g2.view, want2, out_bound(want2, sc.abs() * bnd + U32 * want2.abs(), g2.view.dtype) + 1e-300,
+                          loc, what + " out2")
         g2.check(what + " out2 guard")
     if st is not None:
         u = v.view(M, N // 64, 64)
         want = torch.stack([u.sum(-1), (u * u).sum(-1)], -1).reshape(M, N // 64 * 2)
-        assert_exact(st.view, round_to(want, torch.float32), lambda r, c: f"row {r} unit {c // 2}", what + " ln_stats")
+        if bnd is None:
+            assert_exact(st.view, round_to(want, torch.float32), unit, what + " ln_stats")
+        else:   # four fp32 chains of 16 per unit, combined (test_gpu_kernels._producer_check)
+            ub = bnd.view(M, N // 64, 64)
+            b1 = ub.sum(-1) + 64 * U32 * u.abs().sum(-1)
+            b2 = (2 * u.abs() * ub + ub * ub).sum(-1) + 66 * U32 * (u * u).sum(-1)
+            assert_within(st.view, want, torch.stack([b1, b2], -1).reshape(M, N // 64 * 2) + 1e-300, unit,
+                          what + " ln_stats")
         st.check(what + " ln_stats guard")
+    if act:
+        _check_slices(ops, A, W, kw, g_out, g2, st, so, s2, r if resid == "alias" else None,
+                      dict(M=M, N=N, tile=64 if conv_grouped else tile, rpb=rpb, nb=nb, batched=batched, lens=lens,
+                           stats=stats, sa_buf=sa_buf, resid_sep=r if resid == "sep" else None), loc, what)
+
+
+def _check_blocks(g, gs, want, bnd, loc, what):
+    """Block-scaled e4m3 output: codes g [M, N] and scales gs [N/64][M].  bnd None: codes and scales equal the scale
+    rule of `want` bitwise (masked rows without a residual are zero with scale 1); else (`want` inexact) the dequantised
+    output is within half an e4m3 ulp of the scale plus bnd, and every nonzero unit's largest code is in [224, 448]."""
+    from f5_tts_mlx_b200.weights import quantize_e4m3_blocks
+    M, N = g.view.shape
+    if bnd is None:
+        q, sc = quantize_e4m3_blocks(want, 64)
+        assert_exact(gs.view.T.contiguous(), sc, lambda r, c: f"row {r} unit {c}", what + " scales")
+        assert_exact(g.view, q, loc, what + " codes")
+    else:
+        codes = g.view.view(F8).double().view(M, N // 64, 64)
+        sc = gs.view.T.double()
+        deq = (codes * sc[..., None]).view(M, N)
+        b = bnd + U_E4M3 * (want.abs() + bnd) + E4M3_SUB * sc.repeat_interleave(64, 1)
+        assert_within(deq, want, b, loc, what + " dequantised")
+        amax = codes.abs().amax(-1)
+        nz = want.abs().view(M, N // 64, 64).amax(-1) > 0
+        assert ((amax >= 224) & (amax <= 448))[nz].all(), what + ": a unit's largest code is outside [224, 448]"
+    gs.check(what + " scale guard")
+
+
+def _check_slices(ops, A, W, kw, g_out, g2, st, so, s2, r_alias, geo, loc, what):
+    """(b) of run_exact's activation check: the same GEMM as sub-launches of at most SMs tiles each.  Flat rows are cut at
+    128-row boundaries; utterances (batched or conv mode, or a row mask) are kept whole.  Every sub-launch gets views
+    with row offsets into A, out, out2, resid, ln_stats, ln_in_stats, a_scale (its ld kept) and row_len, and its own
+    [N/64][rows] scale buffers, concatenated for the comparison."""
+    M, N, tile, rpb, nb = geo["M"], geo["N"], geo["tile"], geo["rpb"], geo["nb"]
+    sms = _sm_count()
+    if rpb:      # whole utterances, as many per slice as fit in one wave
+        cuts, b = [], 0
+        while b < nb:
+            e = b + 1
+            while e < nb and gemm_tile_count(N, (e + 1 - b) * rpb, tile, rows_per_batch=rpb, num_batches=e + 1 - b,
+                                             batched=geo["batched"]) <= sms:
+                e += 1
+            cuts.append((b * rpb, e * rpb, b, e))
+            b = e
+    else:
+        step = (sms // cdiv(N, tile)) * 128
+        assert step > 0
+        cuts = [(r0, min(r0 + step, M), 0, 1) for r0 in range(0, M, step)]
+    out_s = torch.empty(g_out.view.shape, dtype=g_out.view.dtype, device=DEV)
+    if r_alias is not None:
+        out_s.copy_(r_alias)
+    out2_s = torch.empty(g2.view.shape, dtype=g2.view.dtype, device=DEV) if g2 is not None else None
+    st_s = torch.empty(st.view.shape, dtype=torch.float32, device=DEV) if st is not None else None
+    so_s, s2_s = [], []
+    for r0, r1, b0, b1 in cuts:
+        m = r1 - r0
+        t = gemm_tile_count(N, m, tile, rows_per_batch=rpb if rpb else 0, num_batches=b1 - b0 if rpb else 1,
+                            batched=geo["batched"])
+        assert t <= sms, f"slice rows [{r0}, {r1}) has {t} tiles > {sms} SMs"
+        k = dict(kw)
+        if rpb:
+            k["num_batches"] = b1 - b0
+        if geo["lens"] is not None:
+            k["row_len"] = geo["lens"][b0:b1]
+        if "resid" in k:
+            k["resid"] = out_s[r0:r1] if r_alias is not None else geo["resid_sep"][r0:r1]
+        if geo["stats"] is not None:
+            k["ln_in_stats"] = geo["stats"][r0:r1]
+        if geo["sa_buf"] is not None:
+            k["a_scale"] = geo["sa_buf"][:, r0:]
+        if out2_s is not None:
+            k["out2"] = out2_s[r0:r1]
+        if st_s is not None:
+            k["ln_stats"] = st_s[r0:r1].view(m, N // 64, 2)
+        if so is not None:
+            so_s.append(torch.empty(N // 64, m, device=DEV))
+            k["out_scale"] = so_s[-1]
+        if s2 is not None:
+            s2_s.append(torch.empty(N // 64, m, device=DEV))
+            k["out2_scale"] = s2_s[-1]
+        ops.gemm(A[r0:r1], W, out_s[r0:r1], out_fp8=g_out.view.dtype == torch.uint8, **k)
+    torch.cuda.synchronize()
+    sl = what + f" vs {len(cuts)} one-wave slices"
+    assert_exact(g_out.view, out_s, loc, sl + " out")
+    if out2_s is not None:
+        assert_exact(g2.view, out2_s, loc, sl + " out2")
+    if st_s is not None:
+        assert_exact(st.view, st_s, lambda r_, c_: f"row {r_} unit {c_ // 2}", sl + " ln_stats")
+    if so is not None:
+        assert_exact(so.view, torch.cat(so_s, 1), lambda u_, r_: f"unit {u_} row {r_}", sl + " out scales")
+    if s2 is not None:
+        assert_exact(s2.view, torch.cat(s2_s, 1), lambda u_, r_: f"unit {u_} row {r_}", sl + " out2 scales")
 
 
 def inst_of(c: dict) -> tuple:
-    return instantiation(act=0, out_dtype={"bf16": torch.bfloat16, "f32": torch.float32, "e4m3": torch.uint8}[c.get("out", "bf16")],
-                         rope=c.get("rope", False), fp8=c.get("ab8", False) or c.get("out") == "e4m3" or c.get("out2") == "e4m3",
-                         resid=c.get("resid") is not None, tile=c["tile"])
+    """The instantiation (kernel_check.instantiation) a run_exact case launches."""
+    scaled = c.get("scaled", False) or c.get("out_blocks", False)
+    fp8 = c.get("ab8", False) or scaled or c.get("out") == "e4m3" or c.get("out2") == "e4m3"
+    return instantiation(act=c.get("act", 0),
+                         out_dtype={"bf16": torch.bfloat16, "f32": torch.float32, "e4m3": torch.uint8}[c.get("out", "bf16")],
+                         rope=c.get("rope", False), fp8=fp8, resid=c.get("resid") is not None, tile=c["tile"],
+                         conv_grouped=c.get("conv_grouped", False), scaled=scaled)
 
 
 # ---------------------------------------------------------------- shape grid (flat, bias only)

@@ -162,3 +162,52 @@ def test_every_instantiation_has_gpu_cases_at_each_tile_width():
     # every instantiation at both tile widths (only the grouped convolution is limited to 64, and none is grouped-only)
     missing = sorted((i, bn) for i in built for bn in (64, 128) if i + (bn,) not in declared)
     assert not missing, f"instantiations without a GPU case: {missing}"
+
+
+def test_launch_geometry_restates_the_launcher():
+    """kernel_check's tile width and tile count follow f5_gemm_bf16 (gemm.cu) on known answers."""
+    from kernel_check import gemm_bn, gemm_num_kb, gemm_tile_count
+    assert gemm_bn(1024, 1874, sms=132) == 128                    # 15 x 8 = 120 tiles >= 107: 128 wide
+    assert gemm_bn(1024, 937, sms=132) == 64                      # 8 x 8 = 64 < 107
+    assert gemm_bn(64, 100000, sms=132) == 64 and gemm_bn(100, 128, tile_n=128, sms=132) == 128
+    assert gemm_bn(512, 300, tile_n=128, conv_grouped=True, sms=132) == 64
+    assert gemm_bn(1024, 3 * 300, rows_per_batch=300, num_batches=3, batched=True, sms=132) == 64   # 3 x 3 x 8 = 72
+    assert gemm_tile_count(1000, 300, 128) == 8 * 3
+    assert gemm_tile_count(1000, 300, 64, rows_per_batch=150, num_batches=2, batched=True) == 16 * 4
+    assert gemm_num_kb(320) == 5 and gemm_num_kb(640, ab8=True) == 5 and gemm_num_kb(64, conv_taps=31) == 31
+    # the restated lines of gemm.cu are still there
+    src = (ROOT / "f5_tts_mlx_b200" / "csrc" / "gemm.cu").read_text()
+    for line in ("if (a->conv_grouped) bn = 64;",
+                 "const int mt = batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128);",
+                 "bn = (mt * cdiv(a->n, 128) >= (sm_count() * 13) / 16 || a->n <= 64) ? 128 : 64;",
+                 "const int tiles = cdiv(a->n, bn) * (batched ? nb * cdiv(rpb, 128) : cdiv(a->m, 128));",
+                 "dim3 grid(std::min(tiles, sm_count()), 1, 1);",
+                 "return dispatch_scaled<64, 6>", "return dispatch_scaled<128, 4>", "return dispatch_epi<64, 6>",
+                 "return dispatch_epi<128, 4>"):
+        assert line in src, line
+
+
+def test_every_instantiation_has_a_many_waves_case():
+    """Every (instantiation, BN) of dispatch_epi and dispatch_scaled has exactly one WAVES case (test_gpu_gemm_persistent)
+    that, on a 132-SM H100, launches more than 3 x 132 tiles (every CTA runs at least 3, on both consumer warpgroups)
+    with num_kb not a multiple of the ring depth.  A new instantiation without such a case fails here, named."""
+    from test_fp8_block import built_scaled_instantiations
+    import test_gpu_gemm_persistent as P
+    from test_gpu_kernel_exact import inst_of
+    sms = 132
+    pairs = {(False,) + i + (bn,) for i in built_instantiations() for bn in (64, 128)}
+    pairs |= {(True,) + i + (bn,) for i in built_scaled_instantiations() for bn in (64, 128)}
+    assert len(pairs) == 36
+    covered = {}
+    for name in P.WAVES:
+        c = P.wave_case(name, sms)
+        geo = P.wave_geometry(c, sms)
+        key = (c.get("scaled", False) or c.get("out_blocks", False),) + inst_of(c)
+        assert key in pairs, f"{name}: launches {key}, which gemm.cu does not build"
+        assert key[-1] == geo["bn"], (name, geo)
+        assert key not in covered, f"{name} and {covered.get(key)} both cover {key}"
+        assert 3 * sms < geo["tiles"] < 4 * sms and geo["per_cta"][0] >= 3, (name, geo)
+        assert geo["num_kb"] % geo["stages"] != 0, (name, geo)
+        covered[key] = name
+    missing = sorted(pairs - set(covered))
+    assert not missing, f"(SCALED, ACT, OUT_BF16, ROPE, FP8, RESID, BN) without a many-waves case: {missing}"
