@@ -13,21 +13,10 @@
 #include "host_common.h"
 #include "launch.h"
 
-extern "C" int f5_attention_fwd(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
-                                int32_t, const int32_t*, void*);
-extern "C" int f5_attention_fwd_e4m3(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
-                                     int32_t, const int32_t*, void*);
-extern "C" int f5_attention_fwd_e4m3_scaled(const void*, int64_t, void*, int64_t, int32_t, int32_t, int32_t,
-                                            int32_t, const int32_t*, float*, void*);
-extern "C" int f5_qkv_quant_e4m3_masked(const void*, int64_t, void*, int64_t, void*, int64_t, float*, int32_t,
-                                        int32_t, int32_t, const int32_t*, void*);
-extern "C" int f5_attention_fwd_fp8(const void*, int64_t, const void*, int64_t, const float*, void*, int64_t, int32_t,
-                                    int32_t, int32_t, int32_t, const int32_t*, float*, void*);
-
 namespace f5 {
 
-static f5_gemm_args gemm_base(const void* a, int64_t lda, const void* w, int64_t ldw, int m, int n,
-                              int k, void* out, int64_t ldo, bool out_bf16) {
+f5_gemm_args gemm_args(const void* a, int64_t lda, const void* w, int64_t ldw, int m, int n, int k, void* out,
+                       int64_t ldo, bool out_bf16, bool w_static) {
   f5_gemm_args g;
   memset(&g, 0, sizeof(g));
   g.a = a; g.lda = lda; g.w = w; g.ldw = ldw;
@@ -36,9 +25,51 @@ static f5_gemm_args gemm_base(const void* a, int64_t lda, const void* w, int64_t
   g.conv_taps = 1;
   g.out = out; g.ldo = ldo; g.out_bf16 = out_bf16 ? 1 : 0;
   g.q_scale = 1.f;
-  g.w_static = 1;   // every W on this path is a model weight
+  g.w_static = w_static ? 1 : 0;
   return g;
 }
+
+f5_gemm_args conv_pos_args(const void* a, const void* w, const float* bias, void* out, bool out_bf16, int D, int N,
+                           int batches, bool w_static) {
+  f5_gemm_args g = gemm_args(a, D, w, 31 * 64, batches * N, D, 64, out, D, out_bf16, w_static);
+  g.bias = bias; g.act = F5_ACT_MISH;
+  g.rows_per_batch = N; g.num_batches = batches; g.batched_tiles = 1;
+  g.conv_taps = 31; g.conv_pad = 15; g.conv_grouped = 1;
+  return g;
+}
+
+template <typename Weights, typename Buffers>
+int text_embedding(const Weights* w, const Buffers* b, int batch_out, int drop_from, int mask_padding,
+                   const int* valid_len, const int* row_len, bool w_static, cudaStream_t st) {
+  const int N = b->frames, R = batch_out * N, C = w->text_dim, Ci = w->text_inner;
+  if (int e = launch_text_embed_gather(b->text, b->batch, b->text_len_max, N, C, w->text_emb, w->text_pos,
+                                       w->text_max_pos, b->text_x, batch_out, drop_from, st, mask_padding, valid_len))
+    return e;
+  for (int l = 0; l < w->conv_layers; ++l) {
+    const f5_convnext_weights& cw = w->text_blocks[l];
+    if (int e = launch_dwconv7_ln(b->text_x, b->text_a, batch_out, N, C, cw.dw_w, cw.dw_b, cw.ln_w, cw.ln_b, st))
+      return e;
+    {  // pwconv1 + exact GELU (convnext_v2.py:50-51)
+      f5_gemm_args g = gemm_args(b->text_a, C, cw.pw1_w, C, R, Ci, C, b->text_h, Ci, true, w_static);
+      g.bias = cw.pw1_b; g.act = F5_ACT_GELU_ERF;
+      if (int e = f5_gemm_bf16(&g, st)) return e;
+    }
+    if (int e = launch_grn(b->text_h, b->text_g, b->grn_nx, cw.grn_gamma, cw.grn_beta, batch_out, N, Ci, st,
+                           valid_len))
+      return e;
+    {  // pwconv2 + residual, then the re-mask of dit.py:225 (masked rows have a zero residual)
+      f5_gemm_args g = gemm_args(b->text_g, Ci, cw.pw2_w, Ci, R, C, Ci, b->text_x, C, false, w_static);
+      g.bias = cw.pw2_b; g.resid = b->text_x; g.ldr = C;
+      if (row_len) { g.rows_per_batch = N; g.num_batches = batch_out; g.row_len = row_len; }
+      if (int e = f5_gemm_bf16(&g, st)) return e;
+    }
+  }
+  return 0;
+}
+template int text_embedding(const f5_dit_weights*, const f5_dit_buffers*, int, int, int, const int*, const int*, bool,
+                            cudaStream_t);
+template int text_embedding(const f5_duration_weights*, const f5_duration_buffers*, int, int, int, const int*,
+                            const int*, bool, cudaStream_t);
 
 // What f5_dit_forward runs, chosen by the buffers the caller binds (see f5_dit_buffers in include/f5_b200.h)
 struct DitMode {
@@ -118,6 +149,101 @@ static long long ln_tab_ld(const f5_dit_weights* w) {
   return (long long)w->depth * (3 * w->dim + w->ff_inner) + 128;
 }
 
+// What one of a block's four GEMMs reads in the current mode
+struct GemmOperands {
+  const void* a;
+  const void* w;             // the bf16 weight, or its e4m3 copy
+  int ab_fp8;
+  float acc_scale;           // per-tensor FP8: the weight's scale; block-scaled: 1; bf16: unused (0)
+  const float* a_scale;      // block-scaled FP8: A's per-(row, 64-column unit) scales
+  const float* w_scale;      // block-scaled FP8: the weight's per-channel scales
+  const void* prefetch;      // weights of the next GEMM to pull into L2, or NULL
+  int64_t prefetch_bytes;
+};
+struct BlockOperands { GemmOperands qkv, out, ff1, ff2; };
+
+// FP8 mode: the QKV / FF1 operand is written as e4m3 by the producing epilogue, the out-projection / FF2 operand
+// (attention output / GELU output) by its producer into the first half of the bf16 buffer.  Block-scaled FP8
+// (DESIGN.md section 8) adds per-channel weight scales and per-(row, 64-column unit) activation scales.
+static BlockOperands block_operands(const f5_dit_weights* w, const f5_dit_buffers* b, const DitMode& m, int l,
+                                    bool prefetch) {
+  const f5_dit_block_weights& k = w->blocks[l];
+  auto pick = [&](const void* a16, const void* a8, const void* w16, const void* w8, float s8, const float* ws,
+                  const float* a_scale) {
+    GemmOperands o = {};
+    o.a = m.fp8 ? a8 : a16;
+    o.w = m.fp8 ? w8 : w16;
+    o.ab_fp8 = m.fp8 ? 1 : 0;
+    o.acc_scale = m.blk8 ? 1.f : m.fp8 ? s8 : 0.f;
+    if (m.blk8) { o.a_scale = a_scale; o.w_scale = ws; }
+    return o;
+  };
+  BlockOperands o = {pick(b->a_bf16, b->a_fp8, k.qkv_w, k.qkv_w8, k.qkv_s8, k.qkv_ws, b->a_fp8_scale),
+                     pick(b->c_bf16, b->c_bf16, k.out_w, k.out_w8, k.out_s8, k.out_ws, b->attn_scale),
+                     pick(b->a_bf16, b->a_fp8, k.ff1_w, k.ff1_w8, k.ff1_s8, k.ff1_ws, b->a_fp8_scale),
+                     pick(b->ff_bf16, b->ff_bf16, k.ff2_w, k.ff2_w8, k.ff2_s8, k.ff2_ws, b->ff_scale)};
+  // weight prefetch chain (L2): each GEMM pulls in the next one's weights, FF2 the next block's QKV weights.
+  // The per-tensor FP8 mode prefetches the bf16 copies, which it does not read.
+  auto fetch = [&](GemmOperands& g, const void* w16, const void* w8, int64_t elems) {
+    if (!prefetch) return;
+    g.prefetch = m.blk8 ? w8 : w16;
+    g.prefetch_bytes = m.blk8 ? elems : 2 * elems;
+  };
+  const int64_t D = w->dim, F = w->ff_inner;
+  fetch(o.qkv, k.out_w, k.out_w8, D * D);
+  fetch(o.out, k.ff1_w, k.ff1_w8, F * D);
+  fetch(o.ff1, k.ff2_w, k.ff2_w8, D * F);
+  if (l + 1 < w->depth) fetch(o.ff2, w->blocks[l + 1].qkv_w, w->blocks[l + 1].qkv_w8, 3 * D * D);
+  return o;
+}
+
+// A [m, k] and W [n, k] dense
+static f5_gemm_args block_gemm(const GemmOperands& o, int m, int n, int k, void* out, int64_t ldo, bool out_bf16) {
+  f5_gemm_args g = gemm_args(o.a, k, o.w, k, m, n, k, out, ldo, out_bf16, true);
+  g.ab_fp8 = o.ab_fp8; g.acc_scale = o.acc_scale;
+  if (o.a_scale) { g.a_scale = o.a_scale; g.a_scale_ld = m; }
+  g.w_scale = o.w_scale;
+  g.prefetch = o.prefetch; g.prefetch_bytes = o.prefetch_bytes;
+  return g;
+}
+
+// Fused AdaLN, producer side: the GEMM writing the residual stream also writes the next LayerNorm's operand
+// x * (1 + ln_scale), as e4m3 (with its block scales in the block-scaled mode) when the next GEMM reads e4m3
+static void ln_producer(f5_gemm_args& g, const DitMode& m, const f5_dit_buffers* b, int D, const float* ln_scale,
+                        bool e4m3) {
+  if (!m.fused) return;
+  g.ln_scale = ln_scale; g.ln_stats = b->ln_stats;
+  g.out2_bf16 = e4m3 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = e4m3 ? 1 : 0;
+  if (e4m3 && m.blk8) g.out2_scale = b->a_fp8_scale;
+}
+
+// Fused AdaLN, consumer side: the GEMM normalises its A operand with the producer's statistics and the c1 / c2 rows of
+// time ti, from ln_tab column `col` on
+static void ln_consumer(f5_gemm_args& g, const DitMode& m, const f5_dit_weights* w, const f5_dit_buffers* b, int ti,
+                        long long col) {
+  if (!m.fused) return;
+  g.ln_in_stats = b->ln_stats; g.ln_tab = b->ln_tab + (size_t)4 * ti * ln_tab_ld(w) + col; g.ln_tab_ld = ln_tab_ld(w);
+}
+
+// attention of b->qkv_bf16 into b->c_bf16: bf16 output, or e4m3 for the FP8 modes' out-projection
+static int attention(const f5_dit_weights* w, const f5_dit_buffers* b, const DitMode& m, int BU, cudaStream_t st) {
+  const int D = w->dim, N = b->frames;
+  const int32_t* kv_len = b->seq_len ? b->seq_len : b->valid_len;   // the pass and the attention mask alike
+  if (m.attn8) {
+    const int64_t vt_ld = (int64_t)cdiv(N, 128) * 128;
+    if (int e = f5_qkv_quant_e4m3_masked(b->qkv_bf16, 3 * D, b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, BU, N,
+                                         w->heads, kv_len, st))
+      return e;
+    return f5_attention_fwd_fp8(b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, b->c_bf16, D, BU, N, w->heads, 64,
+                                kv_len, b->attn_scale, st);
+  }
+  if (m.blk8)
+    return f5_attention_fwd_e4m3_scaled(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64, kv_len, b->attn_scale,
+                                        st);
+  return (m.fp8 ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
+                                                            kv_len, st);
+}
+
 }  // namespace f5
 
 using namespace f5;
@@ -132,38 +258,19 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
   const int D = w->dim, N = b->frames, B = b->batch;
   const int BU = (b->cfg ? 2 : 1) * B;  // row-utterances
   const int R = BU * N;
-  const int C = w->text_dim, Ci = w->text_inner;
+  const int C = w->text_dim;
 
   // ---- TextEmbedding (dit.py:196-229) for the cond rows and, with CFG, the text-dropped rows ----
-  if (int e = launch_text_embed_gather(b->text, B, b->text_len_max, N, C, w->text_emb, w->text_pos,
-                                       w->text_max_pos, b->text_x, BU,
-                                       b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU), st, 1, b->valid_len))
+  if (int e = text_embedding(w, b, BU, b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU), 1, b->valid_len, b->text_len,
+                             true, st))
     return e;
-  for (int l = 0; l < w->conv_layers; ++l) {
-    const f5_convnext_weights& cw = w->text_blocks[l];
-    if (int e = launch_dwconv7_ln(b->text_x, b->text_a, BU, N, C, cw.dw_w, cw.dw_b, cw.ln_w, cw.ln_b, st))
-      return e;
-    {  // pwconv1 + exact GELU (convnext_v2.py:50-51)
-      f5_gemm_args g = gemm_base(b->text_a, C, cw.pw1_w, C, R, Ci, C, b->text_h, Ci, true);
-      g.bias = cw.pw1_b; g.act = F5_ACT_GELU_ERF;
-      if (int e = f5_gemm_bf16(&g, st)) return e;
-    }
-    if (int e = launch_grn(b->text_h, b->text_g, b->grn_nx, cw.grn_gamma, cw.grn_beta, BU, N, Ci, st, b->valid_len))
-      return e;
-    {  // pwconv2 + residual, then the re-mask of dit.py:225 (masked rows have a zero residual)
-      f5_gemm_args g = gemm_base(b->text_g, Ci, cw.pw2_w, Ci, R, C, Ci, b->text_x, C, false);
-      g.bias = cw.pw2_b; g.resid = b->text_x; g.ldr = C;
-      g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->text_len;
-      if (int e = f5_gemm_bf16(&g, st)) return e;
-    }
-  }
 
   // ---- hoisted part of InputEmbedding.proj (dit.py:248-249): [cond | text] · W[:,100:]^T + b ----
   if (int e = launch_concat_cond_text(b->cond, w->mel_dim, B, N, b->text_x, C, b->ct_bf16, w->ct_ld,
                                       R, b->cfg ? B * N : ((b->drop_flags & 1) ? 0 : R), st))
     return e;
   {
-    f5_gemm_args g = gemm_base(b->ct_bf16, w->ct_ld, w->in_ct_w, w->ct_ld, R, D, w->ct_ld, b->hoist, D, false);
+    f5_gemm_args g = gemm_args(b->ct_bf16, w->ct_ld, w->in_ct_w, w->ct_ld, R, D, w->ct_ld, b->hoist, D, false, true);
     g.bias = w->in_b;
     if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }   // bucket rows stay 0
     if (int e = f5_gemm_bf16(&g, st)) return e;
@@ -175,7 +282,7 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
     return e;
   {
     const int NM = w->depth * 6 * D + 2 * D;
-    f5_gemm_args g = gemm_base(b->silu_t, D, w->mod_w, D, b->n_times, NM, D, b->mod_table, NM, false);
+    f5_gemm_args g = gemm_args(b->silu_t, D, w->mod_w, D, b->n_times, NM, D, b->mod_table, NM, false, true);
     g.bias = w->mod_b;
     g.tile_n = 128;
     if (int e = f5_gemm_bf16(&g, st)) return e;
@@ -192,7 +299,8 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
       if (site == 2 * w->depth) { wt = w->proj_w; n = w->mel_dim; off = (long long)w->depth * (3 * D + F); }
       else if (site & 1) { wt = w->blocks[l].ff1_w; n = F; off = (long long)l * (3 * D + F) + 3 * D; }
       else { wt = w->blocks[l].qkv_w; n = 3 * D; off = (long long)l * (3 * D + F); }
-      f5_gemm_args g = gemm_base(prep + (size_t)site * 4 * T * D, D, wt, D, 4 * T, n, D, b->ln_tab + off, ld, false);
+      f5_gemm_args g =
+          gemm_args(prep + (size_t)site * 4 * T * D, D, wt, D, 4 * T, n, D, b->ln_tab + off, ld, false, true);
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
   }
@@ -214,17 +322,10 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
   // weight prefetch chain: worthwhile while a GEMM's weights are comparable to its activations
   // (small batch); at large batch the activations evict them anyway and HBM is busy
   const bool prefetch = R <= 16384;
-  // FP8 mode: all four block GEMMs on e4m3 weights; the QKV / FF1 operand is written as e4m3 by the producing
-  // epilogue, the out-projection / FF2 operand (attention output / GELU output) by its producer into the first half of
-  // the bf16 buffer.  Block-scaled FP8 (DESIGN.md section 8) adds per-channel weight scales and per-(row, 64-column
-  // unit) activation scales.
-  const bool fused = mode.fused, fp8 = mode.fp8, blk8 = mode.blk8;
-  const long long tab_ld = ln_tab_ld(w);
-  const float* tab = fused ? b->ln_tab + (size_t)4 * ti * tab_ld : nullptr;   // this time's 4 operand rows
 
   // ---- InputEmbedding (dit.py:249-251): x·Wx + hoist, then + ConvPositionEmbedding ----
   {
-    f5_gemm_args g = gemm_base(b->y_bf16, 128, w->in_x_w, 128, R, D, 128, b->h, D, false);
+    f5_gemm_args g = gemm_args(b->y_bf16, 128, w->in_x_w, 128, R, D, 128, b->h, D, false, true);
     g.resid = b->hoist; g.ldr = D;
     g.out2_bf16 = b->a_bf16; g.ldo2 = D;
     // bucket rows (>= valid_len): x·Wx masked to 0 + hoist (0 there) = 0 — the conv below sees the reference's zero padding
@@ -232,121 +333,61 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
   {
-    f5_gemm_args g = gemm_base(b->a_bf16, D, w->conv_w[0], 31 * 64, R, D, 64, b->c_bf16, D, true);
-    g.bias = w->conv_b[0]; g.act = F5_ACT_MISH;
-    g.rows_per_batch = N; g.num_batches = BU; g.batched_tiles = 1;
-    g.conv_taps = 31; g.conv_pad = 15; g.conv_grouped = 1;
+    f5_gemm_args g = conv_pos_args(b->a_bf16, w->conv_w[0], w->conv_b[0], b->c_bf16, true, D, N, BU, true);
     g.row_len = b->valid_len;      // NULL, or: the second conv's input is zero on bucket rows too
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
   {
-    f5_gemm_args g = gemm_base(b->c_bf16, D, w->conv_w[1], 31 * 64, R, D, 64, b->x, D, false);
-    g.bias = w->conv_b[1]; g.act = F5_ACT_MISH;
-    g.rows_per_batch = N; g.num_batches = BU; g.batched_tiles = 1;
-    g.conv_taps = 31; g.conv_pad = 15; g.conv_grouped = 1;
+    f5_gemm_args g = conv_pos_args(b->c_bf16, w->conv_w[1], w->conv_b[1], b->x, false, D, N, BU, true);
     g.resid = b->h; g.ldr = D;
-    if (fused) {   // the stream's first producer: operand + statistics for block 0's attn_norm
-      g.ln_scale = (w->depth > 0 ? mod + D : mod + (size_t)w->depth * 6 * D); g.ln_stats = b->ln_stats;
-      g.out2_bf16 = fp8 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = fp8 ? 1 : 0;
-      if (blk8) g.out2_scale = b->a_fp8_scale;
-    }
+    ln_producer(g, mode, b, D, mod + D, mode.fp8);   // the stream's first producer: block 0's attn_norm
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
 
   // ---- transformer blocks (dit.py:311-325) ----
   for (int l = 0; l < w->depth; ++l) {
     const f5_dit_block_weights& bw = w->blocks[l];
+    const BlockOperands op = block_operands(w, b, mode, l, prefetch);
     const float* m = mod + (size_t)l * 6 * D;  // shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
-    if (!fused)
+    const bool last = l + 1 == w->depth;
+    if (!mode.fused)
       if (int e = launch_ln_modulate(b->x, b->a_bf16, R, D, 0, m + D, m, 0, 1, st)) return e;
     {
-      f5_gemm_args g = gemm_base(b->a_bf16, D, bw.qkv_w, D, R, 3 * D, D, b->qkv_bf16, 3 * D, true);
+      f5_gemm_args g = block_gemm(op.qkv, R, 3 * D, D, b->qkv_bf16, 3 * D, true);
       g.bias = bw.qkv_b;
-      if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)l * (3 * D + F); g.ln_tab_ld = tab_ld; }
-      if (fp8) { g.a = b->a_fp8; g.w = bw.qkv_w8; g.ab_fp8 = 1; g.acc_scale = bw.qkv_s8; }
-      if (blk8) { g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.qkv_ws; g.acc_scale = 1.f; }
+      ln_consumer(g, mode, w, b, ti, (long long)l * (3 * D + F));
       g.rows_per_batch = N; g.num_batches = BU;
       g.rope = b->rope; g.rope_cols = 2 * D; g.q_scale = 0.125f; g.q_cols = D;
-      // weight prefetch chain (L2): while QKV runs, pull in out_w and ff1_w (contiguous in the pack)
-      if (prefetch) { g.prefetch = bw.out_w; g.prefetch_bytes = (int64_t)2 * D * D; }
-      if (prefetch && blk8) { g.prefetch = bw.out_w8; g.prefetch_bytes = (int64_t)D * D; }   // the e4m3 weights it reads
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
-    if (mode.attn8) {
-      const int64_t vt_ld = (int64_t)cdiv(N, 128) * 128;
-      const int32_t* kv_len = b->seq_len ? b->seq_len : b->valid_len;   // the pass and the attention mask alike
-      if (int e = f5_qkv_quant_e4m3_masked(b->qkv_bf16, 3 * D, b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, BU,
-                                           N, w->heads, kv_len, st))
-        return e;
-      if (int e = f5_attention_fwd_fp8(b->qk_fp8, 2 * D, b->vt_fp8, vt_ld, b->qkv_scale, b->c_bf16, D, BU, N, w->heads,
-                                       64, kv_len, b->attn_scale, st))
-        return e;
-    } else if (blk8) {
-      if (int e = f5_attention_fwd_e4m3_scaled(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads, 64,
-                                               b->seq_len ? b->seq_len : b->valid_len, b->attn_scale, st))
-        return e;
-    } else if (int e = (fp8 ? f5_attention_fwd_e4m3 : f5_attention_fwd)(b->qkv_bf16, 3 * D, b->c_bf16, D, BU, N, w->heads,
-                                                                         64, b->seq_len ? b->seq_len : b->valid_len, st)) {
-      return e;
-    }
+    if (int e = attention(w, b, mode, BU, st)) return e;
     {
-      f5_gemm_args g = gemm_base(b->c_bf16, D, bw.out_w, D, R, D, D, b->x, D, false);
+      f5_gemm_args g = block_gemm(op.out, R, D, D, b->x, D, false);
       g.bias = bw.out_b;
       g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->seq_len;
       g.gate = m + 2 * D;
       g.resid = b->x; g.ldr = D;
-      if (prefetch) { g.prefetch = bw.ff1_w; g.prefetch_bytes = (int64_t)2 * F * D; }
-      if (fused) {   // ff_norm
-        g.ln_scale = m + 4 * D; g.ln_stats = b->ln_stats;
-        g.out2_bf16 = fp8 ? b->a_fp8 : b->a_bf16; g.ldo2 = D; g.out2_fp8 = fp8 ? 1 : 0;
-      }
-      if (fp8) { g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = bw.out_s8; }     // A = c_bf16's bytes, e4m3 [R, D]
-      if (blk8) {
-        g.w = bw.out_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.out_ws;
-        g.a_scale = b->attn_scale; g.a_scale_ld = R; g.out2_scale = b->a_fp8_scale;
-        if (prefetch) { g.prefetch = bw.ff1_w8; g.prefetch_bytes = (int64_t)F * D; }
-      }
+      ln_producer(g, mode, b, D, m + 4 * D, mode.fp8);   // ff_norm
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
-    if (!fused)
+    if (!mode.fused)
       if (int e = launch_ln_modulate(b->x, b->a_bf16, R, D, 0, m + 4 * D, m + 3 * D, 0, 1, st)) return e;
     {
-      f5_gemm_args g = gemm_base(b->a_bf16, D, bw.ff1_w, D, R, F, D, b->ff_bf16, F, true);
+      f5_gemm_args g = block_gemm(op.ff1, R, F, D, b->ff_bf16, F, true);
       g.bias = bw.ff1_b; g.act = F5_ACT_GELU_TANH;
-      if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)l * (3 * D + F) + 3 * D; g.ln_tab_ld = tab_ld; }
-      if (fp8) {   // out: ff_bf16's bytes as e4m3 [R, F]
-        g.a = b->a_fp8; g.w = bw.ff1_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff1_s8; g.out_fp8 = 1;
-      }
-      if (prefetch) { g.prefetch = bw.ff2_w; g.prefetch_bytes = (int64_t)2 * D * F; }
-      if (blk8) {
-        g.a_scale = b->a_fp8_scale; g.a_scale_ld = R; g.w_scale = bw.ff1_ws; g.acc_scale = 1.f;
-        g.out_fp8 = 1; g.out_scale = b->ff_scale;
-        if (prefetch) { g.prefetch = bw.ff2_w8; g.prefetch_bytes = (int64_t)D * F; }
-      }
+      ln_consumer(g, mode, w, b, ti, (long long)l * (3 * D + F) + 3 * D);
+      g.out_fp8 = mode.fp8 ? 1 : 0;   // FP8: ff_bf16's bytes as e4m3 [R, F], FF2's operand
+      g.out_scale = mode.blk8 ? b->ff_scale : nullptr;
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
     {
-      f5_gemm_args g = gemm_base(b->ff_bf16, F, bw.ff2_w, F, R, D, F, b->x, D, false);
+      f5_gemm_args g = block_gemm(op.ff2, R, D, F, b->x, D, false);
       g.bias = bw.ff2_b;
       g.rows_per_batch = N; g.num_batches = BU;
       g.gate = m + 5 * D;
       g.resid = b->x; g.ldr = D;
-      if (prefetch && l + 1 < w->depth) {
-        g.prefetch = w->blocks[l + 1].qkv_w; g.prefetch_bytes = (int64_t)2 * 3 * D * D;
-      }
-      if (fused) {   // next block's attn_norm scale, or norm_out's (scale first, dit.py:287)
-        g.ln_scale = (l + 1 < w->depth) ? mod + (size_t)(l + 1) * 6 * D + D : mod + (size_t)w->depth * 6 * D;
-        g.ln_stats = b->ln_stats; g.out2_bf16 = b->a_bf16; g.ldo2 = D;
-        if (fp8 && l + 1 < w->depth) { g.out2_bf16 = b->a_fp8; g.out2_fp8 = 1; }   // proj_out (after the last block) stays bf16
-      }
-      if (fp8) { g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = bw.ff2_s8; }
-      if (blk8) {
-        g.w = bw.ff2_w8; g.ab_fp8 = 1; g.acc_scale = 1.f; g.w_scale = bw.ff2_ws;
-        g.a_scale = b->ff_scale; g.a_scale_ld = R;
-        if (g.out2_fp8) g.out2_scale = b->a_fp8_scale;
-        g.prefetch = nullptr; g.prefetch_bytes = 0;
-        if (prefetch && l + 1 < w->depth) { g.prefetch = w->blocks[l + 1].qkv_w8; g.prefetch_bytes = (int64_t)3 * D * D; }
-      }
+      // next block's attn_norm scale, or norm_out's (scale first, dit.py:287); proj_out's operand stays bf16
+      ln_producer(g, mode, b, D, last ? mod + (size_t)w->depth * 6 * D : m + 6 * D + D, mode.fp8 && !last);
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
   }
@@ -354,11 +395,11 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
   // ---- AdaLayerNormZero_Final (scale first, dit.py:287) + proj_out (dit.py:398-399) ----
   {
     const float* mf = mod + (size_t)w->depth * 6 * D;
-    if (!fused)
+    if (!mode.fused)
       if (int e = launch_ln_modulate(b->x, b->a_bf16, R, D, 0, mf, mf + D, 0, 1, st)) return e;
-    f5_gemm_args g = gemm_base(b->a_bf16, D, w->proj_w, D, R, w->mel_dim, D, b->v, w->mel_dim, false);
+    f5_gemm_args g = gemm_args(b->a_bf16, D, w->proj_w, D, R, w->mel_dim, D, b->v, w->mel_dim, false, true);
     g.bias = w->proj_b;
-    if (fused) { g.ln_in_stats = b->ln_stats; g.ln_tab = tab + (size_t)w->depth * (3 * D + F); g.ln_tab_ld = tab_ld; }
+    ln_consumer(g, mode, w, b, ti, (long long)w->depth * (3 * D + F));
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
   return 0;

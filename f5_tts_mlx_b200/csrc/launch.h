@@ -41,4 +41,20 @@ int launch_concat_cond_text(const float* cond, int dc, int Bc, int N, const floa
 int launch_ln_tab_prep(const float* mod, void* prep_bf16, int T, int L, int D, int NM, cudaStream_t st);
 int launch_duration_head(const float* x, int B, int N, int D, const int* len, const float* norm_w,
                          const float* pred_w, float* out, cudaStream_t st);
+
+// ---- host-side stages shared by the DiT (dit.cu, where they are defined) and the duration predictor ----
+// f5_gemm_args of out = A·W^T with every optional field off; w_static as f5_gemm_args.w_static
+f5_gemm_args gemm_args(const void* a, int64_t lda, const void* w, int64_t ldw, int m, int n, int k, void* out,
+                       int64_t ldo, bool out_bf16, bool w_static);
+// one grouped k=31 conv of ConvPositionEmbedding (dit.py:33-38), Mish(conv(a) + bias), over `batches` utterances of
+// N frames; the caller adds the second conv's residual
+f5_gemm_args conv_pos_args(const void* a, const void* w, const float* bias, void* out, bool out_bf16, int D, int N,
+                           int batches, bool w_static);
+// TextEmbedding (dit.py:196-229) on f5_dit_* or f5_duration_* weights and buffers: the gather of `batch_out`
+// utterances into b->text_x (text-dropped from drop_from on), then each ConvNeXtV2 block: dwconv7 + LayerNorm,
+// pwconv1 + exact GELU, GRN (over valid_len frames, NULL = all) and pwconv2 + residual, whose rows at or beyond
+// row_len are written as zeros (row_len NULL: none)
+template <typename Weights, typename Buffers>
+int text_embedding(const Weights* w, const Buffers* b, int batch_out, int drop_from, int mask_padding,
+                   const int* valid_len, const int* row_len, bool w_static, cudaStream_t st);
 }  // namespace f5
