@@ -42,6 +42,25 @@ def _resolve(path_or_repo: str, quantization_bits: Optional[int]) -> Optional[Pa
         return None
 
 
+def checkpoint_weights(path: Path, quantization_bits: Optional[int] = None, convert_weights=None):
+    """(vocab, weights_fn) of a local model directory as from_pretrained reads it: weights_fn() returns the DiT's
+    weights with the reference's parameter names (converted from the upstream keys, or dequantised)."""
+    from safetensors.torch import load_file
+    vocab = read_vocab(path / "vocab.txt")
+    convert = True if convert_weights is None else convert_weights               # cfm.py:455
+    model_file = "model_v1.safetensors"
+    if quantization_bits is not None:                                            # cfm.py:450-453
+        model_file, convert = f"model_v1_{quantization_bits}b.safetensors", False
+
+    def weights_fn() -> Weights:
+        w = load_file(str(path / model_file))
+        if quantization_bits is not None:     # nn.quantize + load_weights (cfm.py:510-517): dense again at pack time
+            return dequantize_mlx_checkpoint(w, quantization_bits)
+        return convert_upstream_keys(w) if convert else w
+
+    return vocab, weights_fn
+
+
 def _resolve_vocos(model_dir: Optional[Path]) -> Optional[Path]:
     """The vocoder checkpoint: next to the model, $F5_VOCOS_PATH (file or directory), or the hub repo the reference
     uses (cfm.py:446)."""
@@ -126,20 +145,9 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
     if path is None:
         raise ValueError(f"Could not find model {hf_model_name_or_path}")        # cfm.py:413-414
     from safetensors.torch import load_file
-    vocab = read_vocab(path / "vocab.txt")
-    convert = True if convert_weights is None else convert_weights               # cfm.py:455
-    model_file = "model_v1.safetensors"
-    if quantization_bits is not None:                                            # cfm.py:450-453
-        model_file, convert = f"model_v1_{quantization_bits}b.safetensors", False
+    vocab, weights_fn = checkpoint_weights(path, quantization_bits, convert_weights)
     dit = DiT(dim=1024, depth=22, heads=16, ff_mult=2, text_dim=512, conv_layers=4,
               text_num_embeds=len(vocab) - 1, text_mask_padding=True, device=device, **fp8_kw)     # cfm.py:459-469
-
-    def weights_fn() -> Weights:
-        w = load_file(str(path / model_file))
-        if quantization_bits is not None:     # nn.quantize + load_weights (cfm.py:510-517): dense again at pack time
-            return dequantize_mlx_checkpoint(w, quantization_bits)
-        return convert_upstream_keys(w) if convert else w
-
     load_weights_distributed(dit, weights_fn)
     if vocoder is None:                                                          # cfm.py:446: always present
         vpath = _resolve_vocos(path)

@@ -72,10 +72,14 @@ def linear(x: Tensor, w: Tensor, b: Optional[Tensor], prec: Precision = FP32) ->
 def adaln_linear(x: Tensor, scale: Tensor, shift: Tensor, w: Tensor, b: Optional[Tensor], prec: Precision = FP32,
                  eps: float = 1e-6, fp8_scale: Optional[float] = None) -> Tensor:
     """Linear(LayerNorm(x) * (1 + scale) + shift) — dit.py:270 + the Linear that consumes it (dit.py:136-143, 94,
-    398).  fp32: exactly that.  With `prec.ln_by_linearity` it applies the CUDA path's rounding points: the
-    producer GEMM's epilogue stores bf16(x * (1 + scale)) and per-row (mean, M2); the consumer GEMM multiplies that
-    operand and finishes the LayerNorm in its epilogue by linearity,
-        out = rstd * (x~ @ W^T - mean * c1) + c2,   c1 = (1 + scale) @ W^T,  c2 = shift @ W^T + b   (fp32 tables)."""
+    398).  fp32: exactly that.  With `prec.ln_by_linearity` it applies the CUDA path's operand rounding point: the
+    producer GEMM's epilogue stores bf16(x * (1 + scale)) and the consumer GEMM multiplies that operand and finishes
+    the LayerNorm in its epilogue by linearity,
+        out = rstd * (x~ @ W^T - mean * c1) + c2,   c1 = (1 + scale) @ W^T,  c2 = shift @ W^T + b   (fp32 tables).
+    The mean and rstd here are exact two-pass statistics of x.  The kernels do not compute those: the producer stores
+    the fp32 (sum, sum of squares) of every 64-column unit and the consumer forms var = E[x^2] - mean^2 from them,
+    whose error grows like r^2 with r = |mean| / std (tests/adaln_emul.py emulates that; below r ~ 1000 at D = 1024
+    the operand rounding, which this emulation does include, dominates)."""
     d = x.shape[-1]
     if not (prec.emulate_bf16 and prec.ln_by_linearity):
         norm = F.layer_norm(x, (d,), eps=eps) * (1 + scale[:, None]) + shift[:, None]

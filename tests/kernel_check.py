@@ -326,3 +326,101 @@ def attention_bound(o: torch.Tensor, pv: torch.Tensor, qk_abs: torch.Tensor, log
         + 2 * tiles * (EPS_EX2 + U32)
     b = 2 * d * pv + 2 * U32 * (tiles * 128 + 1) * pv + 3 * U32 * o.abs()
     return out_bound(o, b, out_dtype)
+
+
+# ---------------------------------------------------------------- fused AdaLN (LayerNorm finished in the GEMM epilogue)
+EPS_LN = float(torch.tensor(1e-6, dtype=torch.float32))   # the kernels' 1e-6f
+U_HILO = 2.0 ** -16       # |a - hi - lo| <= 2^-8 |a - hi| <= 2^-16 |a| for hi = bf16(a), lo = bf16(a - hi)
+
+
+def fused_ln_stats_bound(x: torch.Tensor):
+    """(mean, var, rstd, dr, dmean) per row [M, 1] of the producer's float64 rows x [M, K], with the bound dr on the
+    relative error of the rstd and dmean on the error of the mean that the fused-LN consumer forms.
+
+    The producer adds each 64-column unit in four chains of 8 per 32 columns, the second 32 continuing chain 0 and
+    two combining levels after each half: at most 20 roundings per element, the squares by fma (one rounding each
+    step).  The consumer adds the K / 64 unit values in unit order.  So |dS1| <= gam(20 + n) sum |x| and
+    |dS2| <= gam(20 + n) sum x^2 (n = K / 64); 1 / K is a power of two.  var = E[x^2] - mean^2 then loses the mean's
+    error twice, and the square, the subtraction and the eps add round once each:
+        dvar <= dE2 + (2 |mean| + dmean) dmean + 3u (E[x^2] + dE2 + eps).
+    With zeta = dvar / (var + eps) < 1 the rsqrt of the perturbed argument is within zeta / (2 (1 - zeta)^1.5) of
+    rstd relatively, and rsqrtf adds 2 ulp.  zeta grows like n u r^2 with r = |mean| / std: this is the cancellation of
+    E[x^2] - mean^2.  At zeta >= 1 the bound is infinite (the variance may cancel to zero and be clamped)."""
+    M, K = x.shape
+    n = K // 64
+    g = (20 + n) * U32 / (1 - (20 + n) * U32)
+    mean = x.mean(-1, keepdim=True)
+    var = ((x - mean) ** 2).mean(-1, keepdim=True)
+    rstd = 1 / torch.sqrt(var + EPS_LN)
+    ex2 = (x * x).mean(-1, keepdim=True)
+    dmean = g * x.abs().mean(-1, keepdim=True)
+    dex2 = g * ex2
+    dvar = dex2 + (2 * mean.abs() + dmean) * dmean + 3 * U32 * (ex2 + dex2 + EPS_LN)
+    zeta = dvar / (var + EPS_LN)
+    dr = torch.where(zeta < 1, zeta / (2 * (1 - zeta.clamp(max=0.999)) ** 1.5), torch.full_like(zeta, math.inf))
+    return mean, var, rstd, dr + 2.0 ** -22 + U32, dmean
+
+
+def fused_ln_ref_bound(x: torch.Tensor, bx: torch.Tensor, s: torch.Tensor, b: torch.Tensor, w: torch.Tensor,
+                       bias: torch.Tensor, acc_err: torch.Tensor, *, op_err: torch.Tensor | None = None,
+                       operand: torch.Tensor | None = None, w_eff: torch.Tensor | None = None):
+    """float64 v = Linear(LayerNorm(x) (1 + s) + b) + bias before the consumer's activation / RoPE, for the
+    producer's float64 rows x [M, K] (within bx [M, K] of the kernel's fp32 x), and the bound on the fused-LN
+    consumer's fp32 value of it:  rstd (x~ W~^T - mean c1) + c2 with c1 = (1 + s) w^T, c2 = b w^T + bias from the
+    hi / lo table of the bf16 weight w [N, K], x~ the producer's operand (bf16 / e4m3 / block-scaled e4m3 of
+    x (1 + s)) and W~ the weight the GEMM multiplies (w, or its dequantised e4m3 copy w_eff).
+
+    The bound is the sum of
+    * operand: rstd sum_k op_err_k |W~_nk|, op_err >= |x~ - x (1 + s)| (u_op |x (1 + s)|: the rounding is relative to
+      |x|, not to the spread, so this term grows like 1 + r with r = |mean| / std);
+    * weight (FP8 modes): rstd sum_k (|x (1 + s)| + op_err) |W~ - w|_nk, the e4m3 weight against the bf16 one the
+      tables use;
+    * accumulation: rstd acc_err (gemm_acc_bound / gemm_acc_bound_fp8 of the operands, times the weight scale);
+    * statistics: |rstd (x - mean)(1 + s) W~^T| dr + rstd dmean |c1| (fused_ln_stats_bound: E[x^2] - mean^2 from
+      the fp32 unit sums);
+    * tables: c1 = hi + lo rows, each an fp32 product of the split (1 + s) with w: the split leaves U_HILO |1 + s|
+      and the fp32 products 2u (K + 1) of |1 + s| |w|; the epilogue's add hi + lo rounds once (the same for c2, whose
+      c2 + bias adds round twice); that error is multiplied by rstd |mean|;
+    * epilogue: rstd * acc_scale, mean * rstd, the inner fma -mu_r c1 + c2 and the outer fma round once each;
+    * input: the kernel's x is within bx of x; ln_propagate carries that through the LayerNorm.
+    Products of two of these terms are below 1 % of their sum, which the factor 1.01 covers.
+
+    With `operand` (the float64 value of the operand x~ the kernel multiplied) the reference is the consumer's
+    arithmetic on that operand with exact statistics and tables, rstd (x~ W~^T - mean c1) + c2, and the operand and
+    weight terms drop out: a bound at the fp32 level that a wrong table row or wrong statistics exceed."""
+    from hbm_check import ln_propagate
+    x = x.double()
+    K = x.shape[1]
+    a = 1 + s.double()
+    wd = w.float().double()
+    we = wd if w_eff is None else w_eff.double()
+    wa = we.abs()
+    mean, var, rstd, dr, dmean = fused_ln_stats_bound(x)
+    xs = x * a
+    c1 = a @ wd.T
+    c2 = b.double() @ wd.T + bias.double()
+    if operand is None:
+        centred = rstd * ((x - mean) * a) @ we.T
+        v = centred + (b.double() @ wd.T) + bias.double()
+        if w_eff is not None:
+            v = rstd * ((x - mean) * a) @ wd.T + c2
+        xa = xs.abs() + (0 if op_err is None else op_err)
+        bd = rstd * (op_err @ wa.T) if op_err is not None else torch.zeros_like(v)
+        if w_eff is not None:
+            bd = bd + rstd * (xa @ (we - wd).abs().T)
+    else:
+        xt = operand.double()
+        centred = rstd * (xt @ we.T - mean * c1)
+        v = centred + c2
+        xa = xt.abs()
+        bd = torch.zeros_like(v)
+    bd = bd + rstd * acc_err
+    bd = bd + centred.abs() * dr + rstd * dmean * c1.abs()
+    aa, ba = a.abs(), b.double().abs()
+    dc1 = (U_HILO * aa + 4 * U32 * (K + 1) * aa) @ wd.abs().T + U32 * c1.abs()
+    dc2 = (U_HILO * ba + 4 * U32 * (K + 1) * ba) @ wd.abs().T + 2 * U32 * c2.abs()
+    bd = bd + rstd * mean.abs() * dc1 + dc2
+    inner = -rstd * mean * c1 + c2
+    bd = bd + U32 * (rstd * (xa @ wa.T) + 2 * rstd * mean.abs() * c1.abs() + inner.abs() + v.abs())
+    bd = bd + ln_propagate(x, bx, a.expand_as(x)) @ wd.abs().T
+    return v, 1.01 * bd
