@@ -68,12 +68,13 @@ class GemmArgs(C.Structure):
         ("ab_fp8", C.c_int32), ("out2_fp8", C.c_int32), ("acc_scale", C.c_float), ("out_fp8", C.c_int32),
         ("a_scale", C.c_void_p), ("a_scale_ld", C.c_int64), ("w_scale", C.c_void_p), ("out_scale", C.c_void_p),
         ("out2_scale", C.c_void_p),
+        ("rope_col2", C.c_int32),
     ]
 
 
 class DitDims(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("dim", "depth", "heads", "ff_inner", "mel_dim", "text_dim", "conv_layers",
-                                         "text_num_embeds")]
+                                         "text_num_embeds", "text_unmasked", "rope_heads")]
 
 
 class DitShape(C.Structure):

@@ -344,12 +344,13 @@ class F5TTS:
 
     @classmethod
     def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None,
-                        fp8_attention=False):
+                        fp8_attention=False, model_version="v1"):
         """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8);
-        fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well."""
+        fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well; model_version: "v1" or "v0"
+        (F5TTS_Base checkpoints, see pretrained.from_pretrained)."""
         from .pretrained import from_pretrained
         return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8,
-                               fp8_attention=fp8_attention)
+                               fp8_attention=fp8_attention, model_version=model_version)
 
 
 CFM = F5TTS

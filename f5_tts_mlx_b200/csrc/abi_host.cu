@@ -94,6 +94,10 @@ int check_dims(const f5_dit_dims* d) {
   F5_REQUIRE(d->depth > 0 && d->ff_inner > 0 && d->mel_dim > 0 && d->mel_dim <= 128 && d->text_dim % 64 == 0 && d->conv_layers >= 0 &&
                  d->text_num_embeds > 0,
              "f5_dit_dims: bad field");
+  F5_REQUIRE(d->text_unmasked == 0 || d->text_unmasked == 1, "f5_dit_dims: text_unmasked %d is not 0 or 1",
+             d->text_unmasked);
+  F5_REQUIRE(d->rope_heads >= 0 && d->rope_heads <= d->heads, "f5_dit_dims: rope_heads %d not in [0, heads %d]",
+             d->rope_heads, d->heads);
   return 0;
 }
 
@@ -284,6 +288,7 @@ extern "C" int f5_bind_packed_weights(const f5_dit_dims* d, const void* device_b
   }
   w->blocks = blocks;
   w->proj_w = at("proj_w"); w->proj_b = f("proj_b");
+  w->text_unmasked = d->text_unmasked; w->rope_heads = d->rope_heads;
   return 0;
 }
 

@@ -142,6 +142,9 @@ static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b, DitMod
   F5_REQUIRE(w->mel_dim % 4 == 0 && w->mel_dim <= 128, "dit: mel_dim %d", w->mel_dim);
   F5_REQUIRE(w->blocks && w->depth > 0, "dit: no blocks");
   F5_REQUIRE(b->batch > 0 && b->frames > 0 && b->n_times > 0, "dit: bad buffer shape");
+  F5_REQUIRE(w->text_unmasked == 0 || w->text_unmasked == 1, "dit: text_unmasked %d is not 0 or 1", w->text_unmasked);
+  F5_REQUIRE(w->rope_heads >= 0 && w->rope_heads <= w->heads, "dit: rope_heads %d not in [0, heads %d] (0 = all heads)",
+             w->rope_heads, w->heads);
   return check_mode(w, b, mode);
 }
 
@@ -261,8 +264,12 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
   const int C = w->text_dim;
 
   // ---- TextEmbedding (dit.py:196-229) for the cond rows and, with CFG, the text-dropped rows ----
-  if (int e = text_embedding(w, b, BU, b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU), 1, b->valid_len, b->text_len,
-                             true, st))
+  // Unmasked text (mask_padding=False, dit.py:226-227): filler rows keep embed[0] + position through every ConvNeXt
+  // block, text-dropped rows are all filler; only bucket rows (>= valid_len, NULL without bucketing) stay zero, the
+  // depthwise conv's zero padding at N.
+  const int drop_from = b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU);
+  if (int e = text_embedding(w, b, BU, drop_from, w->text_unmasked ? 0 : 1, b->valid_len,
+                             w->text_unmasked ? b->valid_len : b->text_len, true, st))
     return e;
 
   // ---- hoisted part of InputEmbedding.proj (dit.py:248-249): [cond | text] · W[:,100:]^T + b ----
@@ -358,6 +365,8 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
       ln_consumer(g, mode, w, b, ti, (long long)l * (3 * D + F));
       g.rows_per_batch = N; g.num_batches = BU;
       g.rope = b->rope; g.rope_cols = 2 * D; g.q_scale = 0.125f; g.q_cols = D;
+      // rope_heads: only the first heads of q and of k are rotated (q_scale still covers every q head)
+      if (w->rope_heads) { g.rope_cols = 64 * w->rope_heads; g.rope_col2 = D; }
       if (int e = f5_gemm_bf16(&g, st)) return e;
     }
     if (int e = attention(w, b, mode, BU, st)) return e;

@@ -108,6 +108,11 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
     F5_REQUIRE(a->rope_cols % 64 == 0 && a->q_cols % 32 == 0, "f5_gemm_bf16: rope_cols/q_cols");
     F5_REQUIRE(a->act == F5_ACT_NONE && a->out_bf16, "f5_gemm_bf16: rope epilogue is bf16/no-act");
   }
+  if (a->rope_col2 != 0)   // second rotated range: whole heads, after the first, inside the matrix
+    F5_REQUIRE(a->rope && a->rope_col2 > 0 && a->rope_col2 % 64 == 0 && a->rope_cols > 0 &&
+                   a->rope_col2 >= a->rope_cols && (int64_t)a->rope_col2 + a->rope_cols <= a->n,
+               "f5_gemm_bf16: rope_col2=%d needs a rope table, a multiple of 64 with rope_cols=%d <= rope_col2 and "
+               "rope_col2 + rope_cols <= n=%d", a->rope_col2, a->rope_cols, a->n);
   if (a->ln_scale) {   // fused-LN producer mode
     F5_REQUIRE(!a->out_bf16 && a->out2_bf16 && a->ln_stats, "f5_gemm_bf16: ln_scale needs an fp32 out, out2_bf16 and ln_stats");
     F5_REQUIRE(a->n % 64 == 0 && !a->rope, "f5_gemm_bf16: ln_scale needs n %% 64 == 0");
@@ -167,6 +172,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   p.row_len = a->row_len;
   p.rope = reinterpret_cast<const float2*>(a->rope);
   p.rope_cols = a->rope_cols;
+  p.rope_col2 = a->rope_col2;
   p.q_scale = a->q_scale;
   p.q_cols = a->q_cols;
   p.out2 = reinterpret_cast<__nv_bfloat16*>(a->out2_bf16);

@@ -27,7 +27,8 @@ struct GemmParams {
   const float* gate;       // f32 [N], shared by all utterances, or null
   const int* row_len;      // [num_batches] valid frames per utterance, or null
   const float2* rope;      // [rows_per_batch, 32] (cos, sin), or null
-  int rope_cols;
+  int rope_cols;           // columns [0, rope_cols) are rotated ...
+  int rope_col2;           // ... and [rope_col2, rope_col2 + rope_cols) (0: the same range again)
   float q_scale;
   int q_cols;
   __nv_bfloat16* out2;     // optional bf16 copy of the result
@@ -388,7 +389,8 @@ __device__ __forceinline__ void epi_apply(const uint32_t (&acc)[32], const float
     for (int j = 0; j < 32; ++j) v[j] = mish_fast(v[j]);
   }
   if (ROPE) {
-    if (col0 < p.rope_cols) {
+    // uniform per chunk (heads are 64 columns, so whole chunks); rope_col2 = 0 repeats the first range
+    if (col0 < p.rope_cols || (unsigned)(col0 - p.rope_col2) < (unsigned)p.rope_cols) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const float2 c = cs[HALF * 16 + j];

@@ -155,6 +155,7 @@ class DiT:
 
     def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.0, ff_mult=4, mel_dim=100,
                  text_num_embeds=256, text_dim=None, text_mask_padding=True, conv_layers=0,
+                 pe_attn_head: Optional[int] = None,
                  device: str | torch.device = "cuda", fused_adaln: bool = True, fp8: bool = False,
                  fp8_scaling: str = "tensor", fp8_attention: bool = False):
         if text_dim is None:
@@ -165,13 +166,17 @@ class DiT:
             # the implicit grouped conv reads 64-channel blocks: its dim/16-channel groups must tile them (64 % (dim/16) == 0)
             raise ValueError(f"libf5b200 supports dim 256, 512 or 1024, not {dim}: the conv position embedding's dim/16-channel "
                              "groups must tile 64-channel blocks (see check_common in csrc/dit.cu)")
-        if not text_mask_padding:
-            raise NotImplementedError("text_mask_padding=False is not on the accelerated path")
+        # text_mask_padding=False and pe_attn_head=1 are the F5TTS_Base (v0) model: filler text tokens are not masked,
+        # and only the first head of q and of k is rotated (upstream's pe_attn_head; None = every head)
+        if pe_attn_head is not None and (isinstance(pe_attn_head, bool) or not isinstance(pe_attn_head, int)
+                                         or not 1 <= pe_attn_head <= heads):
+            raise ValueError(f"pe_attn_head must be None (all heads) or an int in 1..{heads}, not {pe_attn_head!r}")
         if dropout != 0.0:
             raise NotImplementedError("inference path: dropout must be 0")
         self.config = DiTConfig(dim=dim, depth=depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult,
                                 mel_dim=mel_dim, text_num_embeds=text_num_embeds, text_dim=text_dim,
-                                conv_layers=conv_layers, text_mask_padding=text_mask_padding)
+                                conv_layers=conv_layers, text_mask_padding=bool(text_mask_padding),
+                                pe_attn_head=pe_attn_head)
         self.dim, self.depth = dim, depth
         # AdaLN LayerNorm+modulate folded into the neighbouring GEMM epilogues (default); False keeps the separate
         # f5_ln_modulate launches (kept for A/B measurements and as a cross-check in the tests)
@@ -224,7 +229,7 @@ class DiT:
     def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int,
                 masked: bool, bucketed: bool = False) -> DitSession:
         key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8, self.fp8_block,
-               self.fp8_attention)
+               self.fp8_attention, self.config.text_mask_padding, self.config.pe_attn_head)
         s = self._sessions.pop(key, None)
         if s is None:
             while len(self._sessions) >= self.session_cache_size:

@@ -141,6 +141,7 @@ def generate(
     fp8_attention: bool = False,
     resample_ref_audio: bool = False,
     output_sample_rate: int = SAMPLE_RATE,
+    model_version: str = "v1",
 ):
     """generate.py:113-244.  Extensions: `f5tts` reuses a loaded model; `batch_sentences=True` runs all
     sentences as ONE ragged `sample()` batch instead of the reference's serial loop
@@ -152,7 +153,9 @@ def generate(
     `fp8_attention` (with fp8="block"): the attention on e4m3 Q, K and V as well.  `resample_ref_audio`: a reference
     clip at any sample rate is RMS-normalised, then resampled to 24 kHz on the GPU (audio.resample, torchaudio's
     default windowed sinc, as upstream F5-TTS does); without it a clip that is not 24 kHz is refused, as in the
-    reference.  `output_sample_rate`: the returned / written waveform is resampled from 24 kHz to this rate."""
+    reference.  `output_sample_rate`: the returned / written waveform is resampled from 24 kHz to this rate.
+    `model_version`: "v1" (default) or "v0" — F5TTS_Base checkpoints (F5TTS.from_pretrained); `model_name` may also name
+    a .safetensors file with vocab.txt beside it."""
     if fp8_attention and fp8 != "block":
         raise ValueError('fp8_attention needs fp8="block"')
     output_sample_rate = int(output_sample_rate)
@@ -160,7 +163,7 @@ def generate(
         raise ValueError(f"output_sample_rate must be positive, got {output_sample_rate}")
     if f5tts is None:
         f5tts = F5TTS.from_pretrained(model_name, quantization_bits=quantization_bits, fp8=fp8,
-                                      fp8_attention=fp8_attention)
+                                      fp8_attention=fp8_attention, model_version=model_version)
     dev = f5tts.transformer.device
     if f5tts._vocoder is None:
         raise ValueError("generate() needs a model with a vocoder (F5TTS(..., vocoder=Vocos(...).decode)); "
@@ -259,6 +262,8 @@ def main(argv=None) -> None:
                    help="accept a reference clip at any sample rate: resample it to 24 kHz on the GPU")
     p.add_argument("--output-sample-rate", type=int, default=SAMPLE_RATE,
                    help="sample rate of the written waveform (resampled on the GPU from 24 kHz)")
+    p.add_argument("--model-version", type=str, default="v1", choices=["v1", "v0"],
+                   help="v0: an F5TTS_Base checkpoint (unmasked text padding, rotary embedding on the first head only)")
     a = p.parse_args(argv)
     if a.fp8_attention and a.fp8 != "block":
         p.error("--fp8-attention needs --fp8 block")
@@ -272,7 +277,7 @@ def main(argv=None) -> None:
              ref_audio_path=a.ref_audio, ref_audio_text=a.ref_text, steps=a.steps, method=a.method, cfg_strength=a.cfg,
              sway_sampling_coef=a.sway_coef, speed=a.speed, seed=a.seed, quantization_bits=a.q, output_path=a.output,
              fp8=a.fp8, fp8_attention=a.fp8_attention, resample_ref_audio=a.resample,
-             output_sample_rate=a.output_sample_rate)
+             output_sample_rate=a.output_sample_rate, model_version=a.model_version)
 
 
 if __name__ == "__main__":

@@ -44,6 +44,7 @@ def gemm(
     row_len: torch.Tensor | None = None,   # i32 [num_batches]
     rope: torch.Tensor | None = None,      # f32 [rows_per_batch, 32, 2]
     rope_cols: int = 0,
+    rope_col2: int = 0,                    # nonzero: [rope_col2, rope_col2 + rope_cols) is rotated too
     q_scale: float = 1.0,
     q_cols: int = 0,
     rows_per_batch: int = 0,
@@ -107,7 +108,7 @@ def gemm(
     if rope is not None:
         assert rope.dtype == torch.float32 and rope.is_contiguous()
         g.rope = rope.data_ptr()
-    g.rope_cols, g.q_scale, g.q_cols = rope_cols, q_scale, q_cols
+    g.rope_cols, g.rope_col2, g.q_scale, g.q_cols = rope_cols, rope_col2, q_scale, q_cols
     g.tile_n = tile_n
     g.ab_fp8, g.acc_scale, g.out2_fp8 = int(ab_fp8), float(acc_scale), int(out2_fp8)
     g.w_static = int(w_static)

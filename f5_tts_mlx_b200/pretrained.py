@@ -30,27 +30,52 @@ VOCOS_REPO = "lucasnewman/vocos-mel-24khz"
 VOCOS_FILES = ("vocos.safetensors", "vocos-mel-24khz/model.safetensors", "vocos-mel-24khz/vocos.safetensors")
 
 
-def _resolve(path_or_repo: str, quantization_bits: Optional[int]) -> Optional[Path]:
+# model_version -> (checkpoint file of a model directory, DiT arguments).  Both versions have the same parameter names
+# and shapes, so the version is never guessed from a checkpoint's keys.  v0 is upstream's F5TTS_Base (and the fine-tunes
+# built on it): TextEmbedding(mask_padding=False) and rotary embedding on the first attention head only.
+MODEL_VERSIONS = {
+    "v1": ("model_v1.safetensors", dict(text_mask_padding=True, pe_attn_head=None)),    # cfm.py:459-469
+    "v0": ("model_1200000.safetensors", dict(text_mask_padding=False, pe_attn_head=1)),
+}
+
+
+def model_file_name(model_version: str = "v1", quantization_bits: Optional[int] = None) -> str:
+    """The checkpoint a model directory of this version holds; ValueError for an unknown version, or for quantised v0
+    weights (there are no MLX-quantised v0 files)."""
+    if model_version not in MODEL_VERSIONS:
+        raise ValueError(f"model_version must be one of {tuple(MODEL_VERSIONS)}, not {model_version!r}")
+    if quantization_bits is None:
+        return MODEL_VERSIONS[model_version][0]
+    if model_version != "v1":
+        raise ValueError(f"quantization_bits is only available for model_version='v1' (there are no quantised "
+                         f"{model_version} checkpoints)")
+    return f"model_v1_{quantization_bits}b.safetensors"
+
+
+def _resolve(path_or_repo: str, quantization_bits: Optional[int], model_version: str = "v1") -> Optional[Path]:
     p = Path(path_or_repo)
     if p.is_dir():
         return p
     try:                                               # same behaviour as utils.py:179-192 when online
         from huggingface_hub import snapshot_download  # type: ignore
-        fn = "model_v1.safetensors" if quantization_bits is None else f"model_v1_{quantization_bits}b.safetensors"
+        fn = model_file_name(model_version, quantization_bits)
         return Path(snapshot_download(repo_id=path_or_repo, allow_patterns=[fn, "duration_v2.safetensors", "*.txt"]))
     except Exception:
         return None
 
 
-def checkpoint_weights(path: Path, quantization_bits: Optional[int] = None, convert_weights=None):
+def checkpoint_weights(path: Path, quantization_bits: Optional[int] = None, convert_weights=None,
+                       model_file: Optional[str] = None):
     """(vocab, weights_fn) of a local model directory as from_pretrained reads it: weights_fn() returns the DiT's
-    weights with the reference's parameter names (converted from the upstream keys, or dequantised)."""
+    weights with the reference's parameter names (converted from the upstream keys, or dequantised).  `model_file`:
+    the checkpoint inside `path` (default: the v1 one, model_v1[_{4,8}b].safetensors)."""
     from safetensors.torch import load_file
     vocab = read_vocab(path / "vocab.txt")
     convert = True if convert_weights is None else convert_weights               # cfm.py:455
-    model_file = "model_v1.safetensors"
+    if model_file is None:
+        model_file = model_file_name("v1", quantization_bits)
     if quantization_bits is not None:                                            # cfm.py:450-453
-        model_file, convert = f"model_v1_{quantization_bits}b.safetensors", False
+        convert = False
 
     def weights_fn() -> Weights:
         w = load_file(str(path / model_file))
@@ -114,14 +139,20 @@ def convert_vocos_upstream(w: Weights) -> Weights:
 
 def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits: Optional[int] = None,
                     device: str | torch.device = "cuda", vocab_path: Optional[str] = None, vocoder=None,
-                    fp8: Optional[str] = None, fp8_attention: bool = False):
+                    fp8: Optional[str] = None, fp8_attention: bool = False, model_version: str = "v1"):
     """`vocoder`: None = resolve and REQUIRE one (reference behaviour), False = none (sample() returns mels),
     or a callable mel -> waveform.  `fp8`: None = bf16, "tensor" or "block" = the DiT's FP8 mode with that weight /
     activation scaling (DESIGN.md section 8); the weights (dequantised first for quantization_bits) are quantised to
-    e4m3 at pack time.  `fp8_attention` (needs fp8="block"): the attention on e4m3 Q, K and V as well."""
+    e4m3 at pack time.  `fp8_attention` (needs fp8="block"): the attention on e4m3 Q, K and V as well.
+    `model_version`: "v1" (default, the reference's model) or "v0" (upstream's F5TTS_Base and its fine-tunes: unmasked
+    text padding, rotary embedding on the first attention head only; a directory holds model_1200000.safetensors).
+    The version is the caller's to state: v0 and v1 checkpoints have identical keys.  `hf_model_name_or_path` may
+    also name a .safetensors file, with vocab.txt (and optionally duration_v2.safetensors) beside it."""
     import os
     if quantization_bits is not None and quantization_bits not in (4, 8):
         raise ValueError(f"quantization_bits must be 4 or 8 (generate.py --q), got {quantization_bits}")
+    model_file = model_file_name(model_version, quantization_bits)     # ValueError: unknown version, quantised v0
+    version_kw = MODEL_VERSIONS[model_version][1]
     if fp8 is not None and fp8 not in FP8_SCALINGS:
         raise ValueError(f"fp8 must be None or one of {FP8_SCALINGS}, got {fp8!r}")
     fp8_kw = dict(fp8=fp8 is not None, fp8_scaling=fp8 or "tensor", fp8_attention=fp8_attention)
@@ -133,7 +164,8 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
             vocab, vocab_source = ascii_vocab(), "ascii"
         cfg = BASE_CONFIG
         dit = DiT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, ff_mult=cfg.ff_mult, text_dim=cfg.text_dim,
-                  conv_layers=cfg.conv_layers, text_num_embeds=cfg.text_num_embeds, device=device, **fp8_kw)
+                  conv_layers=cfg.conv_layers, text_num_embeds=cfg.text_num_embeds, device=device, **version_kw,
+                  **fp8_kw)
         load_weights_distributed(dit, lambda: random_dit_weights(cfg, seed=1234))
         if vocoder is None:
             vocoder = Vocos(VocosConfig(), device).load_weights(random_vocos_weights()).decode
@@ -141,13 +173,19 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
         m.vocab_source = vocab_source
         return m
 
-    path = _resolve(hf_model_name_or_path, quantization_bits)
+    given = Path(hf_model_name_or_path)
+    if given.is_file():                  # a checkpoint file (fine-tunes have their own names), vocab.txt beside it
+        if given.suffix != ".safetensors":
+            raise ValueError(f"{given} is not a .safetensors checkpoint")
+        path, model_file = given.parent, given.name
+    else:
+        path = _resolve(hf_model_name_or_path, quantization_bits, model_version)
     if path is None:
         raise ValueError(f"Could not find model {hf_model_name_or_path}")        # cfm.py:413-414
     from safetensors.torch import load_file
-    vocab, weights_fn = checkpoint_weights(path, quantization_bits, convert_weights)
+    vocab, weights_fn = checkpoint_weights(path, quantization_bits, convert_weights, model_file)
     dit = DiT(dim=1024, depth=22, heads=16, ff_mult=2, text_dim=512, conv_layers=4,
-              text_num_embeds=len(vocab) - 1, text_mask_padding=True, device=device, **fp8_kw)     # cfm.py:459-469
+              text_num_embeds=len(vocab) - 1, device=device, **version_kw, **fp8_kw)     # cfm.py:459-469
     load_weights_distributed(dit, weights_fn)
     if vocoder is None:                                                          # cfm.py:446: always present
         vpath = _resolve_vocos(path)

@@ -33,6 +33,8 @@ class DiTConfig:
     text_dim: int = 512
     conv_layers: int = 4
     text_mask_padding: bool = True
+    # rotary embedding on the first pe_attn_head heads of q and k only (upstream's name; F5TTS_Base v0 = 1), None = all
+    pe_attn_head: Optional[int] = None
 
     @property
     def ff_inner(self) -> int:
@@ -343,6 +345,7 @@ class DitWeightsC(C.Structure):
         ("mod_w", C.c_void_p), ("mod_b", C.c_void_p),
         ("blocks", C.POINTER(DitBlockWeightsC)),
         ("proj_w", C.c_void_p), ("proj_b", C.c_void_p),
+        ("text_unmasked", C.c_int32), ("rope_heads", C.c_int32),
     ]
 
 
@@ -562,6 +565,7 @@ class PackedDiT:
         w.dim, w.depth, w.heads, w.ff_inner = c.dim, c.depth, c.heads, c.ff_inner
         w.mel_dim, w.text_dim, w.text_inner, w.conv_layers = c.mel_dim, c.text_dim, 2 * c.text_dim, c.conv_layers
         w.text_rows, w.text_max_pos, w.ct_ld = c.text_num_embeds + 1, 4096, self.ct_ld
+        w.text_unmasked, w.rope_heads = int(not c.text_mask_padding), c.pe_attn_head or 0
         for n in ("time_w0", "time_b0", "time_w2", "time_b2", "text_emb", "text_pos", "in_x_w", "in_ct_w", "in_b",
                   "mod_w", "mod_b", "proj_w", "proj_b"):
             setattr(w, n, ptr(n))

@@ -137,6 +137,11 @@ typedef struct f5_gemm_args {
   const float* w_scale;
   float* out_scale;
   float* out2_scale;
+  /* Second rotated column range (ABI 2.004): nonzero rotates [rope_col2, rope_col2 + rope_cols) as well as
+   * [0, rope_cols) — the leading heads of q and of k when the QKV GEMM rotates only the first heads (F5TTS_Base v0:
+   * rope_cols = 64 * rope_heads, rope_col2 = D).  A multiple of 64, >= rope_cols, with rope_col2 + rope_cols <= n and a
+   * rope table set.  0 = [0, rope_cols) alone. */
+  int32_t rope_col2;
 } f5_gemm_args;
 
 int f5_gemm_bf16(const f5_gemm_args* args, void* stream);
@@ -303,6 +308,13 @@ typedef struct f5_dit_weights {
   const void* mod_w; const float* mod_b;        /* bf16 [depth*6D+2D, D], fp32 */
   const f5_dit_block_weights* blocks;           /* HOST array [depth] */
   const void* proj_w; const float* proj_b;      /* bf16 [mel_dim, D], fp32 [mel_dim] */
+  /* Model version (ABI 2.004; zero = the v1 DiT that from_pretrained builds, cfm.py:459-469):
+   * text_unmasked 1: TextEmbedding(mask_padding=False) (dit.py:182-229) — filler tokens (id 0) and the rows past the
+   *   text keep the filler embedding + position table and the ConvNeXt blocks run on them without re-zeroing;
+   * rope_heads 1..heads: rotary embedding on the first rope_heads heads of q and of k only (upstream's pe_attn_head;
+   *   F5TTS_Base v0 rotates the first 64 columns of the un-split q and k projections = head 0); 0 = every head. */
+  int32_t text_unmasked;
+  int32_t rope_heads;
 } f5_dit_weights;
 
 /* Caller-allocated device buffers for one sampling session of `batch` utterances padded to
@@ -521,6 +533,9 @@ int f5_vocos_decode(const f5_vocos_weights* w, const f5_vocos_buffers* b, const 
  * ------------------------------------------------------------------------------------------ */
 typedef struct f5_dit_dims {
   int32_t dim, depth, heads, ff_inner, mel_dim, text_dim, conv_layers, text_num_embeds;
+  /* ABI 2.004: copied into f5_dit_weights by f5_bind_packed_weights (see there); 0, 0 = v1, 1, 1 = F5TTS_Base (v0).
+   * The packed layout does not depend on them. */
+  int32_t text_unmasked, rope_heads;
 } f5_dit_dims;
 typedef struct f5_dit_shape {
   int32_t batch, frames, cfg, n_times, text_len_max;
