@@ -72,6 +72,13 @@ class GemmArgs(C.Structure):
     ]
 
 
+class GemmArgsDilated(C.Structure):
+    """f5_gemm_args with the ABI 2.005 field: conv_dilation sits in what was GemmArgs' tail padding, so both mirrors
+    have the same size and GemmArgs stays a valid 2.004 binding.  Pass it as `C.cast(C.pointer(args),
+    C.POINTER(GemmArgs))`."""
+    _fields_ = GemmArgs._fields_ + [("conv_dilation", C.c_int32)]
+
+
 class DitDims(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("dim", "depth", "heads", "ff_inner", "mel_dim", "text_dim", "conv_layers",
                                          "text_num_embeds", "text_unmasked", "rope_heads")]
@@ -136,6 +143,11 @@ SYMBOLS: dict[str, tuple] = {
     "f5_duration_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_mel_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                  C.c_void_p, C.c_int32, C.c_void_p]),
+    "f5_mel_forward_bigvgan": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                         C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "f5_bigvgan_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_bigvgan_act_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_int32, C.c_void_p, C.c_void_p]),
     "f5_resample_table": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int64]),
     "f5_resample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                               C.c_int64, C.c_void_p]),

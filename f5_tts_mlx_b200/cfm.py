@@ -344,13 +344,14 @@ class F5TTS:
 
     @classmethod
     def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None,
-                        fp8_attention=False, model_version="v1"):
+                        fp8_attention=False, model_version="v1", vocoder=None):
         """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8);
         fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well; model_version: "v1" or "v0"
-        (F5TTS_Base checkpoints, see pretrained.from_pretrained)."""
+        (F5TTS_Base checkpoints, see pretrained.from_pretrained); vocoder: None / "vocos" (default) or "bigvgan"
+        (F5TTS_Base_bigvgan checkpoints, see pretrained.from_pretrained)."""
         from .pretrained import from_pretrained
         return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8,
-                               fp8_attention=fp8_attention, model_version=model_version)
+                               fp8_attention=fp8_attention, model_version=model_version, vocoder=vocoder)
 
 
 CFM = F5TTS

@@ -13,8 +13,11 @@ namespace f5 {
 // (audio.py:143-158), * periodic Hann, 1024-pt real FFT, |.|, @ filters^T, log(max(., 1e-5)).
 // filt_t: fp32 [513, n_mels] (transposed filterbank -> coalesced across mel bins).
 // ---------------------------------------------------------------------------------------------
+// BIGVGAN (BigVGAN's mel, upstream F5-TTS get_bigvgan_mel_spectrogram): frame f = samples [f*hop - (1024-hop)/2, +1024)
+// of the REFLECT-padded signal (x[-i] = x[i], x[T-1+i] = x[T-1-i]), magnitude sqrt(re^2 + im^2 + 1e-9).
 constexpr int kMelWarps = 4;
 
+template <bool BIGVGAN>
 __global__ void __launch_bounds__(kMelWarps * 32)
 mel_kernel(const float* __restrict__ audio, int T, const float* __restrict__ window,
            const float* __restrict__ filt_t, int n_mels, int hop, float* __restrict__ out,
@@ -28,7 +31,7 @@ mel_kernel(const float* __restrict__ audio, int T, const float* __restrict__ win
   const int b = blockIdx.y;
   if (f >= frames) return;
   const float* x = audio + (size_t)b * T;
-  const long long s0 = (long long)f * hop - 512;
+  const long long s0 = (long long)f * hop - (BIGVGAN ? (1024 - hop) / 2 : 512);
 
   // z[n] = x[2n] + i x[2n+1], n = 32 r + lane
   float2 a[16];
@@ -36,8 +39,16 @@ mel_kernel(const float* __restrict__ audio, int T, const float* __restrict__ win
   for (int r = 0; r < 16; ++r) {
     const int n = 32 * r + lane;
     const long long i0 = s0 + 2 * n;
-    const float x0 = (i0 >= 0 && i0 < T) ? x[i0] : 0.f;
-    const float x1 = (i0 + 1 >= 0 && i0 + 1 < T) ? x[i0 + 1] : 0.f;
+    float x0, x1;
+    if constexpr (BIGVGAN) {   // reflect padding (the caller guarantees T > (1024 - hop) / 2)
+      const long long j0 = i0 < 0 ? -i0 : (i0 >= T ? 2LL * (T - 1) - i0 : i0);
+      const long long j1 = i0 + 1 < 0 ? -(i0 + 1) : (i0 + 1 >= T ? 2LL * (T - 1) - (i0 + 1) : i0 + 1);
+      x0 = x[j0];
+      x1 = x[j1];
+    } else {
+      x0 = (i0 >= 0 && i0 < T) ? x[i0] : 0.f;
+      x1 = (i0 + 1 >= 0 && i0 + 1 < T) ? x[i0 + 1] : 0.f;
+    }
     const float2 w = reinterpret_cast<const float2*>(window)[n];
     a[r] = make_float2(x0 * w.x, x1 * w.y);
   }
@@ -54,7 +65,8 @@ mel_kernel(const float* __restrict__ audio, int T, const float* __restrict__ win
     const float2 d = make_float2(0.5f * (zk.x - zc.x), 0.5f * (zk.y - zc.y));
     const float2 wd = cmul(twiddle(k, 1024), d);          // W^k * d
     const float re = e.x + wd.y, im = e.y - wd.x;         // e - i * wd
-    mags[warp][k] = sqrtf(re * re + im * im);
+    if constexpr (BIGVGAN) mags[warp][k] = sqrtf(fmaf(re, re, im * im) + 1e-9f);
+    else mags[warp][k] = sqrtf(re * re + im * im);
   }
   __syncwarp();
   for (int m = lane; m < n_mels; m += 32) {
@@ -155,8 +167,26 @@ int f5_mel_forward(const float* audio, int32_t batch, int32_t samples, const flo
   F5_REQUIRE(frames <= samples / hop, "f5_mel_forward: frames %d > samples/hop %d", frames,
              samples / hop);
   ProfScope ps(PROF_OTHER, 0.0, 4.0 * batch * (double)samples + 4.0 * batch * (double)frames * n_mels);
-  F5_CHECK_CUDA(launch_kernel(mel_kernel, dim3(dim3(cdiv(frames, kMelWarps), batch)), dim3(kMelWarps * 32), 0, (cudaStream_t)stream, 
+  F5_CHECK_CUDA(launch_kernel(mel_kernel<false>, dim3(dim3(cdiv(frames, kMelWarps), batch)), dim3(kMelWarps * 32), 0, (cudaStream_t)stream, 
       audio, samples, window, filters, n_mels, hop, out, frames));
+  F5_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int f5_mel_forward_bigvgan(const float* audio, int32_t batch, int32_t samples, const float* window,
+                           const float* filters, int32_t n_mels, int32_t hop, float* out, int32_t frames,
+                           void* stream) {
+  if (int e = device_check()) return e;
+  F5_REQUIRE(audio && window && filters && out, "f5_mel_forward_bigvgan: null pointer");
+  F5_REQUIRE(hop > 0 && hop <= 1024 && (1024 - hop) % 2 == 0, "f5_mel_forward_bigvgan: hop %d", hop);
+  const int pad = (1024 - hop) / 2;
+  F5_REQUIRE(batch > 0 && n_mels > 0 && samples > pad, "f5_mel_forward_bigvgan: reflect padding of %d needs more "
+             "than %d samples, got %d", pad, pad, samples);
+  F5_REQUIRE(frames == (samples + 2 * pad - 1024) / hop + 1, "f5_mel_forward_bigvgan: frames %d != %d", frames,
+             (samples + 2 * pad - 1024) / hop + 1);
+  ProfScope ps(PROF_OTHER, 0.0, 4.0 * batch * (double)samples + 4.0 * batch * (double)frames * n_mels);
+  F5_CHECK_CUDA(launch_kernel(mel_kernel<true>, dim3(dim3(cdiv(frames, kMelWarps), batch)), dim3(kMelWarps * 32), 0,
+                              (cudaStream_t)stream, audio, samples, window, filters, n_mels, hop, out, frames));
   F5_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

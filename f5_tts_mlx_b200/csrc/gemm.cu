@@ -102,6 +102,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   const bool batched = a->batched_tiles != 0;
   F5_REQUIRE(taps == 1 || batched, "f5_gemm_bf16: conv mode requires batched_tiles");
   F5_REQUIRE(!a->conv_grouped || a->k == 64, "f5_gemm_bf16: grouped conv needs k == 64");
+  F5_REQUIRE(a->conv_dilation >= 0, "f5_gemm_bf16: conv_dilation=%d < 0", a->conv_dilation);
   F5_REQUIRE((int64_t)nb * rpb == a->m, "f5_gemm_bf16: m=%d != num_batches*rows_per_batch=%d*%d",
              a->m, nb, rpb);
   if (a->rope) {
@@ -165,6 +166,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   p.conv_pad = a->conv_pad;
   p.k_per_tap = a->k;
   p.conv_grouped = a->conv_grouped;
+  p.conv_dilation = a->conv_dilation;
   p.bias = a->bias;
   p.out = a->out; p.ldo = (int)a->ldo;
   p.resid = a->resid; p.ldr = (int)a->ldr;

@@ -59,6 +59,7 @@ struct GemmParams {
   const float* w_scale;    // [N]: per-output-channel weight scale (multiplies acc_scale), or null
   float* out_scale;        // [N/64][M]: with out_fp8, `out` is quantised per (row, 64-column unit) and the scales written
   float* out2_scale;       // [N/64][M]: the same for out2 (out2_fp8)
+  int conv_dilation;       // implicit-conv mode: frames between taps (0 or 1: adjacent frames)
 };
 
 // Each CTA touches its 1/num_ctas slice of [pf_ptr, pf_ptr + pf_bytes) with L2 prefetches (one warp,

@@ -17,8 +17,8 @@
 //
 // The same kernel runs the 1-D convolutions of the path as implicit GEMMs: the A operand is a
 // 3-D tensor map (channels, frames, batch) and k-block kb reads the tile shifted by
-// (tap - pad) frames; TMA zero-fills the out-of-range frames, which is exactly the conv's zero
-// padding (reference: nn.Conv1d(padding=k//2), dit.py:33-38).
+// (tap * dilation - pad) frames; TMA zero-fills the out-of-range frames, which is exactly the conv's zero
+// padding (reference: nn.Conv1d(padding=k//2), dit.py:33-38; dilation > 1: BigVGAN's AMP-block convolutions).
 //
 // Epilogue (all fp32, fused, per reference op):
 //   v = acc + bias[col]                                   Linear bias        (dit.py:136-143 ...)
@@ -170,6 +170,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
         constexpr int KBE = decltype(ab8_tag)::value ? 128 : 64;     // elements per k-block, compile-time in the loop
         // incremental stage / phase / tap bookkeeping: no division in the loop
         const int kb_per_tap = (p.k_per_tap + KBE - 1) / KBE, num_kb = p.conv_taps * kb_per_tap, tiles = gemm_tiles(p, BN);
+        const int tap_step = p.conv_dilation > 1 ? p.conv_dilation : 1;
         int s = 0;
         uint32_t ph = 1;
         uint8_t* sa = smem;
@@ -177,15 +178,15 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tma_a,
         for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
           const GemmTile g = gemm_tile(p, t, BN);
           const int a_col0 = p.conv_grouped ? g.n0 : 0;
-          const int a_row0 = g.m_in_batch0 - p.conv_pad;
-          int tap = 0, kc = 0;
+          // tap t reads frames m + t * conv_dilation - conv_pad (conv_dilation 0 or 1: m + t - conv_pad)
+          int a_row = g.m_in_batch0 - p.conv_pad, kc = 0;
           for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(&empty_bar[s], ph);
             if (kb >= early) mbar_expect_tx(&full_bar[s], S::kStageBytes);
-            tma_load_3d(sa, &tma_a, &full_bar[s], a_col0 + kc * KBE, a_row0 + tap, g.batch);
+            tma_load_3d(sa, &tma_a, &full_bar[s], a_col0 + kc * KBE, a_row, g.batch);
             if (kb >= early) tma_load_2d(sa + S::kABytes, &tma_b, &full_bar[s], kb * KBE, g.n0);
             if (++s == kStages) { s = 0; ph ^= 1; sa = smem; } else { sa += S::kStageBytes; }
-            if (++kc == kb_per_tap) { kc = 0; ++tap; }
+            if (++kc == kb_per_tap) { kc = 0; a_row += tap_step; }
           }
           early = 0;
         }

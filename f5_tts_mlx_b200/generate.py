@@ -142,6 +142,7 @@ def generate(
     resample_ref_audio: bool = False,
     output_sample_rate: int = SAMPLE_RATE,
     model_version: str = "v1",
+    vocoder: Literal["vocos", "bigvgan"] = "vocos",
 ):
     """generate.py:113-244.  Extensions: `f5tts` reuses a loaded model; `batch_sentences=True` runs all
     sentences as ONE ragged `sample()` batch instead of the reference's serial loop
@@ -155,7 +156,11 @@ def generate(
     default windowed sinc, as upstream F5-TTS does); without it a clip that is not 24 kHz is refused, as in the
     reference.  `output_sample_rate`: the returned / written waveform is resampled from 24 kHz to this rate.
     `model_version`: "v1" (default) or "v0" — F5TTS_Base checkpoints (F5TTS.from_pretrained); `model_name` may also name
-    a .safetensors file with vocab.txt beside it."""
+    a .safetensors file with vocab.txt beside it.  `vocoder`: "vocos" (default) or "bigvgan" — an F5TTS_Base_bigvgan
+    model: BigVGAN v2 and its mel front-end, from bigvgan/ next to the model or $F5_BIGVGAN_PATH; it has no duration
+    predictor, so pass `duration` or `estimate_duration`."""
+    if vocoder not in ("vocos", "bigvgan"):
+        raise ValueError(f'vocoder must be "vocos" or "bigvgan", not {vocoder!r}')
     if fp8_attention and fp8 != "block":
         raise ValueError('fp8_attention needs fp8="block"')
     output_sample_rate = int(output_sample_rate)
@@ -163,7 +168,8 @@ def generate(
         raise ValueError(f"output_sample_rate must be positive, got {output_sample_rate}")
     if f5tts is None:
         f5tts = F5TTS.from_pretrained(model_name, quantization_bits=quantization_bits, fp8=fp8,
-                                      fp8_attention=fp8_attention, model_version=model_version)
+                                      fp8_attention=fp8_attention, model_version=model_version,
+                                      **({"vocoder": "bigvgan"} if vocoder == "bigvgan" else {}))
     dev = f5tts.transformer.device
     if f5tts._vocoder is None:
         raise ValueError("generate() needs a model with a vocoder (F5TTS(..., vocoder=Vocos(...).decode)); "
@@ -264,6 +270,8 @@ def main(argv=None) -> None:
                    help="sample rate of the written waveform (resampled on the GPU from 24 kHz)")
     p.add_argument("--model-version", type=str, default="v1", choices=["v1", "v0"],
                    help="v0: an F5TTS_Base checkpoint (unmasked text padding, rotary embedding on the first head only)")
+    p.add_argument("--vocoder", type=str, default="vocos", choices=["vocos", "bigvgan"],
+                   help="bigvgan: an F5TTS_Base_bigvgan model (BigVGAN v2 and its mel; bigvgan/ next to the model)")
     a = p.parse_args(argv)
     if a.fp8_attention and a.fp8 != "block":
         p.error("--fp8-attention needs --fp8 block")
@@ -277,7 +285,8 @@ def main(argv=None) -> None:
              ref_audio_path=a.ref_audio, ref_audio_text=a.ref_text, steps=a.steps, method=a.method, cfg_strength=a.cfg,
              sway_sampling_coef=a.sway_coef, speed=a.speed, seed=a.seed, quantization_bits=a.q, output_path=a.output,
              fp8=a.fp8, fp8_attention=a.fp8_attention, resample_ref_audio=a.resample,
-             output_sample_rate=a.output_sample_rate, model_version=a.model_version)
+             output_sample_rate=a.output_sample_rate, model_version=a.model_version,
+             **({"vocoder": "bigvgan"} if a.vocoder == "bigvgan" else {}))
 
 
 if __name__ == "__main__":

@@ -110,6 +110,23 @@ def _resolve_vocos(model_dir: Optional[Path]) -> Optional[Path]:
     return None
 
 
+def _resolve_bigvgan(model_dir: Optional[Path]) -> Path:
+    """The BigVGAN directory (bigvgan_generator.pt and config.json): $F5_BIGVGAN_PATH, or bigvgan/ next to the model.
+    Local only: there is no hub download."""
+    import os
+    cands = []
+    env = os.environ.get("F5_BIGVGAN_PATH")
+    if env:
+        cands.append(Path(env))
+    if model_dir is not None:
+        cands.append(model_dir / "bigvgan")
+    for c in cands:
+        if (c / "bigvgan_generator.pt").is_file() and (c / "config.json").is_file():
+            return c
+    raise FileNotFoundError(f"no BigVGAN checkpoint found (looked for bigvgan_generator.pt and config.json in "
+                            f"{', '.join(map(str, cands)) or '$F5_BIGVGAN_PATH (unset)'})")
+
+
 def ascii_vocab() -> dict:
     """Printable ASCII, in the file layout read_vocab() expects (trailing '' entry)."""
     chars = [chr(i) for i in range(32, 127)] + [""]
@@ -144,11 +161,26 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
     or a callable mel -> waveform.  `fp8`: None = bf16, "tensor" or "block" = the DiT's FP8 mode with that weight /
     activation scaling (DESIGN.md section 8); the weights (dequantised first for quantization_bits) are quantised to
     e4m3 at pack time.  `fp8_attention` (needs fp8="block"): the attention on e4m3 Q, K and V as well.
+    `vocoder="bigvgan"`: an F5TTS_Base_bigvgan model (upstream's `--vocoder_name bigvgan`): BigVGAN v2 decodes, and the
+    reference clip goes through BigVGAN's mel (bigvgan.BigVGANMelSpec).  bigvgan_generator.pt and config.json are read
+    from $F5_BIGVGAN_PATH or bigvgan/ next to the model (no download); "random" builds the released config with random
+    weights.  No duration predictor is attached, since duration_v2 was trained on the other mel: pass a duration.
+    State model_version="v0" for these checkpoints (nothing is guessed).  `vocoder="vocos"` is the default behaviour.
     `model_version`: "v1" (default, the reference's model) or "v0" (upstream's F5TTS_Base and its fine-tunes: unmasked
     text padding, rotary embedding on the first attention head only; a directory holds model_1200000.safetensors).
     The version is the caller's to state: v0 and v1 checkpoints have identical keys.  `hf_model_name_or_path` may
-    also name a .safetensors file, with vocab.txt (and optionally duration_v2.safetensors) beside it."""
+    also name a .safetensors file, with vocab.txt (and optionally duration_v2.safetensors) beside it, or an upstream
+    training checkpoint .pt (its ema_model_state_dict, read with torch.load(weights_only=True))."""
     import os
+    if vocoder == "vocos":
+        vocoder = None
+    use_bigvgan = isinstance(vocoder, str) and vocoder == "bigvgan"
+    if isinstance(vocoder, str) and not use_bigvgan:
+        raise ValueError(f"vocoder must be \"vocos\", \"bigvgan\", False, None or a callable, not {vocoder!r}")
+    mel_kw = {}
+    if use_bigvgan:
+        from .bigvgan import BigVGANMelSpec
+        mel_kw = dict(mel_spec_module=BigVGANMelSpec())
     if quantization_bits is not None and quantization_bits not in (4, 8):
         raise ValueError(f"quantization_bits must be 4 or 8 (generate.py --q), got {quantization_bits}")
     model_file = model_file_name(model_version, quantization_bits)     # ValueError: unknown version, quantised v0
@@ -167,26 +199,45 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
                   conv_layers=cfg.conv_layers, text_num_embeds=cfg.text_num_embeds, device=device, **version_kw,
                   **fp8_kw)
         load_weights_distributed(dit, lambda: random_dit_weights(cfg, seed=1234))
-        if vocoder is None:
+        if use_bigvgan:
+            from .bigvgan import BigVGAN, BigVGANConfig, random_bigvgan_weights
+            vocoder = BigVGAN(BigVGANConfig(), device).load_weights(random_bigvgan_weights(BigVGANConfig(), seed=1234)).decode
+        elif vocoder is None:
             vocoder = Vocos(VocosConfig(), device).load_weights(random_vocos_weights()).decode
-        m = cls(transformer=dit, vocab_char_map=vocab, vocoder=vocoder or None)
+        m = cls(transformer=dit, vocab_char_map=vocab, vocoder=vocoder or None, **mel_kw)
         m.vocab_source = vocab_source
         return m
 
     given = Path(hf_model_name_or_path)
     if given.is_file():                  # a checkpoint file (fine-tunes have their own names), vocab.txt beside it
-        if given.suffix != ".safetensors":
-            raise ValueError(f"{given} is not a .safetensors checkpoint")
+        if given.suffix not in (".safetensors", ".pt"):
+            raise ValueError(f"{given} is not a .safetensors or .pt checkpoint")
+        if given.suffix == ".pt" and quantization_bits is not None:
+            raise ValueError("quantization_bits applies to MLX .safetensors checkpoints, not to a .pt file")
         path, model_file = given.parent, given.name
     else:
         path = _resolve(hf_model_name_or_path, quantization_bits, model_version)
     if path is None:
         raise ValueError(f"Could not find model {hf_model_name_or_path}")        # cfm.py:413-414
     from safetensors.torch import load_file
-    vocab, weights_fn = checkpoint_weights(path, quantization_bits, convert_weights, model_file)
+    if given.is_file() and given.suffix == ".pt":      # upstream training checkpoint: the EMA weights, upstream keys
+        vocab = read_vocab(path / "vocab.txt")
+
+        def weights_fn() -> Weights:
+            ck = torch.load(str(given), map_location="cpu", weights_only=True)
+            if "ema_model_state_dict" not in ck:
+                raise ValueError(f"{given} has no ema_model_state_dict")
+            return convert_upstream_keys({k: v.float() for k, v in ck["ema_model_state_dict"].items()})
+    else:
+        vocab, weights_fn = checkpoint_weights(path, quantization_bits, convert_weights, model_file)
     dit = DiT(dim=1024, depth=22, heads=16, ff_mult=2, text_dim=512, conv_layers=4,
               text_num_embeds=len(vocab) - 1, device=device, **version_kw, **fp8_kw)     # cfm.py:459-469
     load_weights_distributed(dit, weights_fn)
+    if use_bigvgan:
+        from .bigvgan import BigVGAN, load_checkpoint
+        bcfg, bsd = load_checkpoint(_resolve_bigvgan(path))
+        vocoder = BigVGAN(bcfg, device).load_weights(bsd).decode
+        return cls(transformer=dit, vocab_char_map=vocab, vocoder=vocoder, **mel_kw)
     if vocoder is None:                                                          # cfm.py:446: always present
         vpath = _resolve_vocos(path)
         if vpath is None:

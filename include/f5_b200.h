@@ -142,6 +142,11 @@ typedef struct f5_gemm_args {
    * rope_cols = 64 * rope_heads, rope_col2 = D).  A multiple of 64, >= rope_cols, with rope_col2 + rope_cols <= n and a
    * rope table set.  0 = [0, rope_cols) alone. */
   int32_t rope_col2;
+  /* Dilated implicit convolution (ABI 2.005): with conv_taps > 1, tap t of output frame m reads input frame
+   * m + t * conv_dilation - conv_pad (zero outside the utterance) — nn.Conv1d(dilation=conv_dilation,
+   * padding=conv_pad).  0 or 1 = adjacent frames.  The field occupies what was the struct's tail padding: sizeof is
+   * unchanged, so a zero-initialised 2.004 struct keeps its meaning. */
+  int32_t conv_dilation;
 } f5_gemm_args;
 
 int f5_gemm_bf16(const f5_gemm_args* args, void* stream);
@@ -444,6 +449,14 @@ int f5_mel_forward(const float* audio, int32_t batch, int32_t samples, const flo
                    const float* filters_t, int32_t n_mels, int32_t hop, float* out, int32_t frames,
                    void* stream);
 
+/* BigVGAN's mel (ABI 2.005; upstream F5-TTS get_bigvgan_mel_spectrogram, the front-end of F5TTS_Base_bigvgan):
+ * frames of the REFLECT-padded signal (pad (1024 - hop) / 2 = 384 on each side), non-centred, periodic Hann, real FFT,
+ * magnitude sqrt(re^2 + im^2 + 1e-9), filters_t (Slaney filterbank, transposed), log(max(., 1e-5)).
+ * frames must equal (samples + 2 pad - 1024) / hop + 1, and samples > pad (reflect padding needs them). */
+int f5_mel_forward_bigvgan(const float* audio, int32_t batch, int32_t samples, const float* window,
+                           const float* filters_t, int32_t n_mels, int32_t hop, float* out, int32_t frames,
+                           void* stream);
+
 /* ------------------------------------------------------------------------------------------ *
  * Sample-rate conversion (ABI 2.003) — torchaudio.functional.resample at its defaults (sinc_interp_hann,
  * lowpass_filter_width 6, rolloff 0.99), the resampler upstream F5-TTS puts in front of the mel front-end for
@@ -514,6 +527,89 @@ int f5_istft(const float* h, int64_t ldh, int32_t batch, int32_t frames, const f
              int32_t out_len, void* stream);
 int f5_vocos_decode(const f5_vocos_weights* w, const f5_vocos_buffers* b, const float* mel,
                     float* wave, void* stream);
+
+/* ------------------------------------------------------------------------------------------ *
+ * BigVGAN v2 vocoder (ABI 2.005; NVIDIA's bigvgan_v2_24khz_100band_256x, upstream F5-TTS --vocoder_name bigvgan), resblock
+ * "1" (AMPBlock1) with Snake / SnakeBeta.  Channels-last throughout: an utterance of T frames and C channels is
+ * [T, C] row-major, utterances one after another.
+ *
+ *   conv_pre   Conv1d(num_mels, C0, 7, pad 3): implicit GEMM over the bf16 mel padded to 128 columns, bf16 out
+ *   ups[i]     ConvTranspose1d(C_i, C_i / 2, k_i, stride u_i, pad (k_i - u_i) / 2) as a POLYPHASE implicit conv: output
+ *              frame n u + q only reads input frames n - up_pad .. n - up_pad + up_taps - 1, so with the weights packed
+ *              as up_w[(q, c_out)][tap][c_in] the GEMM's [T, u C_out] fp32 output is exactly [u T, C_out]
+ *   resblocks  x_j = AMPBlock1_j(x) for j < num_kernels, then x = (x_0 + ... + x_{nk-1}) / nk (fp32 sum in j order,
+ *              one IEEE division; bf16 when it feeds the next ups GEMM, fp32 before activation_post)
+ *              AMPBlock1: for m < 3: t = act(x) [bf16]; t = conv1_m(t) [fp32, dilation d_m]; t = act(t) [bf16];
+ *                         x = conv2_m(t) + x [fp32, the GEMM epilogue's residual]
+ *   act_post   anti-aliased activation, fp32 out
+ *   conv_post  Conv1d(C_last, 1, 7, pad 3, bias optional) on the CUDA cores, then tanh (use_tanh_at_final) or
+ *              clamp(-1, 1)
+ *
+ * Anti-aliased activation (Activation1d): per channel, with replicate padding at each utterance's two edges,
+ *     u[m] = 2 sum_j h_up[j] xp[(m + 15 - j) / 2]    (j with m + 15 - j even; xp = x padded by 5 frames each side)
+ *     a[m] = u[m] + sin(alpha u[m])^2 / (beta + 1e-9)                   (Snake: beta = alpha)
+ *     z[n] = sum_j h_down[j] ap[2 n + j]                (ap = a padded by 5 / 6 samples: replicates the ACTIVATED signal)
+ * in one pass: the 2T-long intermediate stays in shared memory.  sin is the accurate sinf.
+ * ------------------------------------------------------------------------------------------ */
+#define F5_BIGVGAN_MAX_UPS 8
+#define F5_BIGVGAN_MAX_KERNELS 4
+
+typedef struct f5_bigvgan_act {
+  const float* alpha;    /* fp32 [C], already exp() of the stored value when snake_logscale */
+  const float* beta;     /* fp32 [C] (SnakeBeta), or NULL (Snake: the divisor is alpha) */
+  const float* h_up;     /* fp32 [12] upsample.filter */
+  const float* h_down;   /* fp32 [12] downsample.lowpass.filter */
+} f5_bigvgan_act;
+
+typedef struct f5_bigvgan_amp_weights {
+  int32_t kernel;                 /* k of every conv of the block */
+  int32_t dilation[3];
+  const void* conv1_w[3];         /* bf16 [C, k * round_up(C, 64)] tap-major: w[o][t * kp + i] = conv.weight[o, i, t] */
+  const float* conv1_b[3];        /* fp32 [C] */
+  const void* conv2_w[3];
+  const float* conv2_b[3];
+  f5_bigvgan_act act[6];          /* activations[0..5]: act[2m] before conv1_m, act[2m + 1] before conv2_m */
+} f5_bigvgan_amp_weights;
+
+typedef struct f5_bigvgan_weights {
+  int32_t num_mels;               /* <= 128 */
+  int32_t num_upsamples;          /* <= F5_BIGVGAN_MAX_UPS */
+  int32_t num_kernels;            /* resblocks per stage, <= F5_BIGVGAN_MAX_KERNELS */
+  int32_t channels0;              /* upsample_initial_channel C0; stage i has C0 >> (i + 1) channels */
+  int32_t use_tanh_at_final;
+  int32_t reserved[3];
+  int32_t up_rate[F5_BIGVGAN_MAX_UPS];
+  int32_t up_taps[F5_BIGVGAN_MAX_UPS];   /* taps of the polyphase packing */
+  int32_t up_pad[F5_BIGVGAN_MAX_UPS];
+  const void* conv_pre_w;         /* bf16 [C0, 7 * 128] tap-major, mel channels padded to 128 */
+  const float* conv_pre_b;        /* fp32 [C0] */
+  const void* up_w[F5_BIGVGAN_MAX_UPS];   /* bf16 [u C_out, up_taps * round_up(C_in, 64)] */
+  const float* up_b[F5_BIGVGAN_MAX_UPS];  /* fp32 [u C_out]: bias[c_out] repeated per phase */
+  const f5_bigvgan_amp_weights* blocks;   /* HOST array [num_upsamples * num_kernels], resblocks.{n} order */
+  f5_bigvgan_act act_post;
+  const float* conv_post_w;       /* fp32 [7, C_last] tap-major */
+  const float* conv_post_b;       /* fp32 [1], or NULL (use_bias_at_final = false) */
+} f5_bigvgan_weights;
+
+/* stage_elems = max(frames * C0, max_i T_i C_i) with T_i = frames * u_0 ... u_i: the per-utterance size of the scratch */
+typedef struct f5_bigvgan_buffers {
+  int32_t batch, frames, reserved[2];
+  int64_t stage_elems;
+  void* mel_bf16;       /* bf16 [batch * frames, 128] */
+  void* a_bf16;         /* bf16 [batch * stage_elems]: GEMM operands */
+  float* x_up;          /* fp32 [batch * stage_elems]: output of the stage's ups GEMM */
+  float* t;             /* fp32 [batch * stage_elems]: conv1 outputs, the activation_post output */
+  float* xk;            /* fp32 [num_kernels][batch * stage_elems]: the resblocks' residual streams */
+} f5_bigvgan_buffers;
+
+/* mel fp32 [batch, frames, num_mels] -> wave fp32 [batch, frames * prod(up_rate)] */
+int f5_bigvgan_decode(const f5_bigvgan_weights* w, const f5_bigvgan_buffers* b, const float* mel, float* wave,
+                      void* stream);
+/* Kernel test entry: the anti-aliased activation on x fp32 [batch, rows_per_batch, channels]; utterance u has lens[u]
+ * frames (int32 device [batch], or NULL = rows_per_batch), rows at or beyond it are not written.  act is a HOST pointer
+ * to device tables.  out: bf16 (out_bf16 = 1) or fp32, the same layout. */
+int f5_bigvgan_act_forward(const float* x, int32_t batch, int32_t rows_per_batch, int32_t channels,
+                           const int32_t* lens, const f5_bigvgan_act* act, int32_t out_bf16, void* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
  * Host utilities for hosts that are not Python (the package's weights.PackedDiT / dit.DitSession / parallel.py do
