@@ -61,7 +61,7 @@ class GemmArgs(C.Structure):
         ("q_scale", C.c_float), ("q_cols", C.c_int32),
         ("tile_n", C.c_int32),
         ("out2_bf16", C.c_void_p), ("ldo2", C.c_int64),
-        ("w_static", C.c_int32),
+        ("w_static", C.c_int32), ("ln_rms", C.c_int32),
         ("prefetch", C.c_void_p), ("prefetch_bytes", C.c_int64),
         ("ln_scale", C.c_void_p), ("ln_stats", C.c_void_p), ("ln_in_stats", C.c_void_p),
         ("ln_tab", C.c_void_p), ("ln_tab_ld", C.c_int64),
@@ -156,6 +156,12 @@ SYMBOLS: dict[str, tuple] = {
     "f5_vocos_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_ode_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_float,
                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_unett_precompute": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_unett_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "f5_unett_ode_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_float,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "f5_unett_time_pack": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32,
+                                     C.c_int32, C.c_int32, C.c_void_p]),
     "f5_packed_weights_bytes": (C.c_int64, [C.POINTER(DitDims)]),
     "f5_pack_weights": (C.c_int, [C.POINTER(DitDims), TENSOR_LOOKUP, C.c_void_p, C.c_void_p]),
     "f5_bind_packed_weights": (C.c_int, [C.POINTER(DitDims), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

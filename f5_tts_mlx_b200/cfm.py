@@ -23,10 +23,6 @@ from .utils import default, exists, lens_to_mask, list_str_to_idx, list_str_to_t
 METHODS = {"euler": 0, "midpoint": 1, "rk4": 2}
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def time_grid(steps: int, sway_sampling_coef: Optional[float]) -> torch.Tensor:
     """cfm.py:377-381 — fp32 grid of `steps` POINTS (steps-1 intervals) with sway warping."""
     t = torch.linspace(0, 1, steps, dtype=torch.float32)
@@ -92,7 +88,7 @@ def odeint_rk4(func, y0, t):
 
 class _Plan:
     """Everything that is fixed for one (batch, frames, steps, method, sway, cfg) combination: the
-    DiT session buffers, ODE state buffers and the captured CUDA graph of precompute + ODE loop."""
+    backbone's (DiT or UNetT) session buffers, ODE state buffers and the captured CUDA graph of precompute + ODE loop."""
 
     def __init__(self, model: "F5TTS", batch: int, frames: int, text_cols: int, steps: int, method: str,
                  sway: Optional[float], cfg_strength: float, masked: bool, keep_trajectory: bool, bucketed: bool = False):
@@ -118,13 +114,8 @@ class _Plan:
         tr = model.transformer
         self.session.c.drop_flags = 0      # DiT.__call__ may have used this cached session with drop flags set
         tr.precompute(self.session)
-        lib = _lib.load()
-        tg = self.t_grid.numpy().ctypes.data_as(C.POINTER(C.c_float))
-        _lib.check(lib.f5_ode_sample(
-            C.byref(tr.packed.c_struct()), C.byref(self.session.c), tg, self.steps, METHODS[self.method],
-            C.c_float(self.cfg_strength), C.c_void_p(self.y.data_ptr()),
-            C.c_void_p(self.trajectory.data_ptr()) if self.trajectory is not None else None,
-            C.c_void_p(self.scratch.data_ptr()) if self.scratch is not None else None, _stream()))
+        tr.ode_sample(self.session, self.t_grid, self.steps, METHODS[self.method], self.cfg_strength, self.y,
+                      self.trajectory, self.scratch)
 
     def capture(self, model: "F5TTS") -> None:
         """Capture precompute + ODE loop into a CUDA graph (an eager pass must have run on this process before:
@@ -346,9 +337,9 @@ class F5TTS:
     def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quantization_bits=None, fp8=None,
                         fp8_attention=False, model_version="v1", vocoder=None):
         """fp8: None (bf16), "tensor" or "block" — the DiT's FP8 mode and its scaling (DESIGN.md section 8);
-        fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well; model_version: "v1" or "v0"
-        (F5TTS_Base checkpoints, see pretrained.from_pretrained); vocoder: None / "vocos" (default) or "bigvgan"
-        (F5TTS_Base_bigvgan checkpoints, see pretrained.from_pretrained)."""
+        fp8_attention (with fp8="block"): the attention on e4m3 Q, K and V as well; model_version: "v1", "v0"
+        (F5TTS_Base checkpoints) or "e2" (E2TTS_Base, the UNetT backbone), see pretrained.from_pretrained; vocoder:
+        None / "vocos" (default) or "bigvgan" (F5TTS_Base_bigvgan checkpoints, see pretrained.from_pretrained)."""
         from .pretrained import from_pretrained
         return from_pretrained(cls, hf_model_name_or_path, convert_weights, quantization_bits, fp8=fp8,
                                fp8_attention=fp8_attention, model_version=model_version, vocoder=vocoder)

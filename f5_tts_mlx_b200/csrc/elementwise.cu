@@ -90,7 +90,8 @@ int launch_text_embed_gather(const int* text, int B, int nt, int N, int C, const
                              const float* pos_table, int max_pos, float* x, int Bout,
                              int drop_from, cudaStream_t st, int mask_padding, const int* valid_len) {
   ProfScope ps(PROF_OTHER, 0.0, 0.0);
-  F5_REQUIRE(text && emb && pos_table && x, "text_embed_gather: null pointer");
+  F5_REQUIRE(text && emb && x, "text_embed_gather: null pointer");
+  F5_REQUIRE(pos_table || max_pos == 0, "text_embed_gather: max_pos %d without a position table", max_pos);
   F5_REQUIRE(C % 4 == 0, "text_embed_gather: C %% 4");
   F5_CHECK_CUDA(launch_kernel(text_embed_gather_kernel, dim3(dim3(N, Bout)), dim3(128), 0, st, text, B, nt, N, C, emb, pos_table,
                                                           max_pos, x, drop_from, mask_padding, valid_len));

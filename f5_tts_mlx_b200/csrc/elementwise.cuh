@@ -249,7 +249,7 @@ grn_apply_kernel(const __nv_bfloat16* __restrict__ h, __nv_bfloat16* __restrict_
 // ---------------------------------------------------------------------------------------------
 // TextEmbedding front (dit.py:196-222): ids+1, truncate/pad to N with 0, text_mask = (id == 0)
 // computed BEFORE the CFG drop, drop -> id 0, Embedding gather, + sinusoid table row
-// min(n, 4095) (rope.py:76-84), masked rows -> 0.  text: int32 [B, nt] (pad -1).
+// min(n, 4095) (rope.py:76-84; pos_table NULL: none), masked rows -> 0.  text: int32 [B, nt] (pad -1).
 // Output x: fp32 [Bout, N, C].  Utterance bo reads text row (bo % B); rows bo >= drop_from are the
 // CFG "uncond" copies (ids dropped to 0, mask still from the real text).  valid_len (frame bucketing,
 // may be NULL): rows n >= valid_len[bo] do not exist in the reference, whose text is truncated to the
@@ -271,13 +271,18 @@ text_embed_gather_kernel(const int* __restrict__ text, int B, int nt, int N, int
   if (bo >= drop_from) id = 0;
   const int p = n < max_pos ? n : max_pos - 1;
   const float4* er = reinterpret_cast<const float4*>(emb + (size_t)id * C);
-  const float4* pr = reinterpret_cast<const float4*>(pos_table + (size_t)p * C);
+  const float4* pr = pos_table != nullptr ? reinterpret_cast<const float4*>(pos_table + (size_t)p * C) : nullptr;
   float4* xo = reinterpret_cast<float4*>(x + ((size_t)bo * N + n) * C);
   for (int i = threadIdx.x; i < C / 4; i += blockDim.x) {
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (!masked) {
-      const float4 e = er[i], q = pr[i];
-      v = make_float4(e.x + q.x, e.y + q.y, e.z + q.z, e.w + q.w);
+      const float4 e = er[i];
+      if (pr != nullptr) {
+        const float4 q = pr[i];
+        v = make_float4(e.x + q.x, e.y + q.y, e.z + q.z, e.w + q.w);
+      } else {   // no position table (UNetT, conv_layers = 0): the embedding row alone
+        v = e;
+      }
     }
     xo[i] = v;
   }
@@ -350,9 +355,10 @@ __global__ void __launch_bounds__(256) cfg_ode_update_kernel(const OdeUpdatePara
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)p.rows * p.d) return;
   const int r = (int)(i / p.d), c = (int)(i - (long long)r * p.d);
-  float k = p.v[(size_t)r * p.ldv + c];
+  const size_t vr = p.v_frames > 0 ? (size_t)r + r / p.v_frames + 1 : (size_t)r;
+  float k = p.v[vr * p.ldv + c];
   if (p.null_row_offset > 0) {
-    const float nu = p.v[(size_t)(r + p.null_row_offset) * p.ldv + c];
+    const float nu = p.v[(vr + p.null_row_offset) * p.ldv + c];
     k = k + (k - nu) * p.cfg_strength;
   }
   float upd = k;

@@ -118,7 +118,10 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
     F5_REQUIRE(!a->out_bf16 && a->out2_bf16 && a->ln_stats, "f5_gemm_bf16: ln_scale needs an fp32 out, out2_bf16 and ln_stats");
     F5_REQUIRE(a->n % 64 == 0 && !a->rope, "f5_gemm_bf16: ln_scale needs n %% 64 == 0");
   }
-  if (a->ln_in_stats) {   // fused-LN consumer mode
+  if (a->ln_rms) {   // RMSNorm consumer mode
+    F5_REQUIRE(a->ln_in_stats && !a->ln_tab && !a->out2_bf16 && taps == 1 && a->k % 128 == 0 && !ab8,
+               "f5_gemm_bf16: ln_rms needs ln_in_stats, no ln_tab, no second output, a plain bf16 GEMM with k %% 128 == 0");
+  } else if (a->ln_in_stats) {   // fused-LN consumer mode
     F5_REQUIRE(a->ln_tab && a->ln_tab_ld >= a->n && !a->out2_bf16 && taps == 1 && a->k % 128 == 0,
                "f5_gemm_bf16: ln_in_stats needs ln_tab (ld >= n), no second output, a plain GEMM with k %% 128 == 0");
   }
@@ -184,6 +187,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   p.ln_scale = a->ln_scale; p.ln_stats = reinterpret_cast<float2*>(a->ln_stats);
   p.ln_in_stats = reinterpret_cast<const float2*>(a->ln_in_stats); p.ln_in_units = a->k / 64;
   p.ln_tab = a->ln_tab; p.ln_tab_ld = a->ln_tab_ld;
+  p.ln_rms = a->ln_rms != 0 ? 1 : 0;
   p.ab8 = ab8 ? 1 : 0; p.acc_scale = ab8 ? a->acc_scale : 1.f; p.out2_fp8 = a->out2_fp8; p.out_fp8 = a->out_fp8;
   p.a_scale = a->a_scale; p.a_scale_ld = a->a_scale_ld; p.w_scale = a->w_scale;
   p.out_scale = a->out_scale; p.out2_scale = a->out2_scale;

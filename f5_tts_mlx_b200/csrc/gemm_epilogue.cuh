@@ -60,6 +60,9 @@ struct GemmParams {
   float* out_scale;        // [N/64][M]: with out_fp8, `out` is quantised per (row, 64-column unit) and the scales written
   float* out2_scale;       // [N/64][M]: the same for out2 (out2_fp8)
   int conv_dilation;       // implicit-conv mode: frames between taps (0 or 1: adjacent frames)
+  // RMSNorm consumer (f5_gemm_args.ln_rms): the row scale is sqrt(K) / max(||x||, 1e-12) from ln_in_stats, no mean
+  // term and no ln_tab (the norm's gain is folded into W)
+  int ln_rms;
 };
 
 // Each CTA touches its 1/num_ctas slice of [pf_ptr, pf_ptr + pf_bytes) with L2 prefetches (one warp,
@@ -115,7 +118,7 @@ __device__ __forceinline__ void epi_stage_cols(const GemmParams& p, int n0, int 
     if constexpr (SC) ws_s[i] = (p.w_scale != nullptr && ok) ? p.acc_scale * p.w_scale[col] : p.acc_scale;
     float b = (p.bias != nullptr && ok) ? p.bias[col] : 0.f;
     float x = (p.ln_scale != nullptr && ok) ? 1.f + p.ln_scale[col] : 1.f;
-    if (p.ln_in_stats != nullptr && ok) {
+    if (p.ln_in_stats != nullptr && ok && !p.ln_rms) {
       const float* t = p.ln_tab + col;
       x = t[0] + t[p.ln_tab_ld];
       b += t[2 * p.ln_tab_ld] + t[3 * p.ln_tab_ld];
@@ -140,6 +143,10 @@ __device__ __forceinline__ void epi_load_ln_row(const GemmParams& p, int row, bo
     s1 += v.z; s2 += v.w;
   }
   const float inv_k = 1.f / (64.f * p.ln_in_units);
+  if (p.ln_rms) {   // RMSNorm: sqrt(K) / max(||x||, 1e-12) = rsqrt(max(sum x^2, 1e-24) / K), finite for an all-zero row
+    rstd = rsqrtf(fmaxf(s2, 1e-24f) * inv_k);
+    return;
+  }
   const float mean = s1 * inv_k;
   rstd = rsqrtf(fmaxf(s2 * inv_k - mean * mean, 0.f) + 1e-6f);
   mu_r = mean * rstd;

@@ -13,6 +13,9 @@ struct OdeUpdateParams {
   float* k_acc; float acc_w; int acc_init; int use_acc;
   __nv_bfloat16* y_bf16; int ld_bf16; long long bf16_copy_row_offset;
   int rows; int d;
+  // UNetT: v holds v_frames + 1 rows per utterance, the time row first, so state row r reads v row r + r / v_frames + 1
+  // (null_row_offset counts v rows); 0 = one v row per state row (the DiT)
+  int v_frames;
 };
 
 

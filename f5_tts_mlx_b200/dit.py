@@ -257,6 +257,16 @@ class DiT:
                                       int(time_index), C.c_void_p(torch.cuda.current_stream().cuda_stream)))
         return s.v
 
+    def ode_sample(self, s: DitSession, t_grid: torch.Tensor, steps: int, method: int, cfg_strength: float,
+                   y: torch.Tensor, trajectory: Optional[torch.Tensor], scratch: Optional[torch.Tensor]) -> None:
+        """f5_ode_sample: the fixed-grid solve on this backbone (t_grid: host fp32)."""
+        tg = t_grid.numpy().ctypes.data_as(C.POINTER(C.c_float))
+        _lib.check(_lib.load().f5_ode_sample(
+            C.byref(self._require_weights().c_struct()), C.byref(s.c), tg, steps, method, C.c_float(cfg_strength),
+            C.c_void_p(y.data_ptr()), C.c_void_p(trajectory.data_ptr()) if trajectory is not None else None,
+            C.c_void_p(scratch.data_ptr()) if scratch is not None else None,
+            C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+
     def __call__(self, x: torch.Tensor, cond: torch.Tensor, text: torch.Tensor, time: torch.Tensor,
                  drop_audio_cond: bool = False, drop_text: bool = False,
                  mask: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -155,8 +155,9 @@ def generate(
     clip at any sample rate is RMS-normalised, then resampled to 24 kHz on the GPU (audio.resample, torchaudio's
     default windowed sinc, as upstream F5-TTS does); without it a clip that is not 24 kHz is refused, as in the
     reference.  `output_sample_rate`: the returned / written waveform is resampled from 24 kHz to this rate.
-    `model_version`: "v1" (default) or "v0" — F5TTS_Base checkpoints (F5TTS.from_pretrained); `model_name` may also name
-    a .safetensors file with vocab.txt beside it.  `vocoder`: "vocos" (default) or "bigvgan" — an F5TTS_Base_bigvgan
+    `model_version`: "v1" (default), "v0" — F5TTS_Base checkpoints — or "e2" — E2TTS_Base, which has no duration
+    predictor: pass `duration` or `estimate_duration` (F5TTS.from_pretrained); `model_name` may also name a .safetensors
+    file with vocab.txt beside it.  `vocoder`: "vocos" (default) or "bigvgan" — an F5TTS_Base_bigvgan
     model: BigVGAN v2 and its mel front-end, from bigvgan/ next to the model or $F5_BIGVGAN_PATH; it has no duration
     predictor, so pass `duration` or `estimate_duration`."""
     if vocoder not in ("vocos", "bigvgan"):
@@ -268,8 +269,9 @@ def main(argv=None) -> None:
                    help="accept a reference clip at any sample rate: resample it to 24 kHz on the GPU")
     p.add_argument("--output-sample-rate", type=int, default=SAMPLE_RATE,
                    help="sample rate of the written waveform (resampled on the GPU from 24 kHz)")
-    p.add_argument("--model-version", type=str, default="v1", choices=["v1", "v0"],
-                   help="v0: an F5TTS_Base checkpoint (unmasked text padding, rotary embedding on the first head only)")
+    p.add_argument("--model-version", type=str, default="v1", choices=["v1", "v0", "e2"],
+                   help="v0: an F5TTS_Base checkpoint (unmasked text padding, rotary embedding on the first head only); "
+                        "e2: an E2TTS_Base checkpoint (UNetT backbone; pass --duration or --estimate-duration)")
     p.add_argument("--vocoder", type=str, default="vocos", choices=["vocos", "bigvgan"],
                    help="bigvgan: an F5TTS_Base_bigvgan model (BigVGAN v2 and its mel; bigvgan/ next to the model)")
     a = p.parse_args(argv)

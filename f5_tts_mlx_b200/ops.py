@@ -59,6 +59,7 @@ def gemm(
     ln_stats: torch.Tensor | None = None,      # f32 [rows, n/64, 2] (sum, sum of squares) per 64 columns
     ln_in_stats: torch.Tensor | None = None,   # f32 [rows, k/64, 2]: consumer mode
     ln_tab: torch.Tensor | None = None,        # f32 [4, >=n] rows c1_hi, c1_lo, c2_hi, c2_lo
+    ln_rms: bool = False,                      # RMSNorm consumer: ln_in_stats without ln_tab, the norm's gain in w
     ab_fp8: bool = False,                      # a and w are e4m3 bytes (uint8 / float8_e4m3fn tensors), k % 128 == 0
     acc_scale: float = 1.0,                    # multiplies the accumulator in FP8 mode (weight tensor scale)
     out2_fp8: bool = False,                    # out2 is written as e4m3 bytes (uint8 tensor)
@@ -121,7 +122,10 @@ def gemm(
     if ln_scale is not None:
         assert ln_scale.dtype == torch.float32 and ln_stats is not None and ln_stats.dtype == torch.float32
         g.ln_scale, g.ln_stats = ln_scale.data_ptr(), ln_stats.data_ptr()
-    if ln_in_stats is not None:
+    if ln_rms:
+        assert ln_in_stats is not None and ln_in_stats.dtype == torch.float32 and ln_tab is None
+        g.ln_rms, g.ln_in_stats = 1, ln_in_stats.data_ptr()
+    elif ln_in_stats is not None:
         assert ln_in_stats.dtype == torch.float32 and ln_tab is not None and ln_tab.dtype == torch.float32
         g.ln_in_stats, g.ln_tab, g.ln_tab_ld = ln_in_stats.data_ptr(), ln_tab.data_ptr(), ln_tab.stride(0)
     for t in (a_scale, w_scale, out_scale, out2_scale):

@@ -36,6 +36,8 @@ VOCOS_FILES = ("vocos.safetensors", "vocos-mel-24khz/model.safetensors", "vocos-
 MODEL_VERSIONS = {
     "v1": ("model_v1.safetensors", dict(text_mask_padding=True, pe_attn_head=None)),    # cfm.py:459-469
     "v0": ("model_1200000.safetensors", dict(text_mask_padding=False, pe_attn_head=1)),
+    # E2TTS_Base: the UNetT backbone (unett.py), upstream's E2TTS_Base/model_1200000.safetensors
+    "e2": ("model_1200000.safetensors", dict(text_mask_padding=False, pe_attn_head=1)),
 }
 
 
@@ -166,12 +168,16 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
     from $F5_BIGVGAN_PATH or bigvgan/ next to the model (no download); "random" builds the released config with random
     weights.  No duration predictor is attached, since duration_v2 was trained on the other mel: pass a duration.
     State model_version="v0" for these checkpoints (nothing is guessed).  `vocoder="vocos"` is the default behaviour.
-    `model_version`: "v1" (default, the reference's model) or "v0" (upstream's F5TTS_Base and its fine-tunes: unmasked
-    text padding, rotary embedding on the first attention head only; a directory holds model_1200000.safetensors).
+    `model_version`: "v1" (default, the reference's model), "v0" (upstream's F5TTS_Base and its fine-tunes: unmasked
+    text padding, rotary embedding on the first attention head only; a directory holds model_1200000.safetensors) or
+    "e2" (upstream's E2TTS_Base on the UNetT backbone: see _from_pretrained_e2).
     The version is the caller's to state: v0 and v1 checkpoints have identical keys.  `hf_model_name_or_path` may
     also name a .safetensors file, with vocab.txt (and optionally duration_v2.safetensors) beside it, or an upstream
     training checkpoint .pt (its ema_model_state_dict, read with torch.load(weights_only=True))."""
     import os
+    if model_version == "e2":
+        return _from_pretrained_e2(cls, hf_model_name_or_path, quantization_bits, device, vocab_path, vocoder, fp8,
+                                   fp8_attention)
     if vocoder == "vocos":
         vocoder = None
     use_bigvgan = isinstance(vocoder, str) and vocoder == "bigvgan"
@@ -256,3 +262,81 @@ def from_pretrained(cls, hf_model_name_or_path: str, convert_weights=None, quant
                                             text_num_embeds=len(vocab) - 1),
             vocab_char_map=vocab, device=device).load_weights(load_file(str(dpath)))
     return cls(transformer=dit, vocab_char_map=vocab, vocoder=vocoder, duration_predictor=duration_predictor)
+
+
+def _from_pretrained_e2(cls, hf_model_name_or_path: str, quantization_bits, device, vocab_path, vocoder, fp8,
+                        fp8_attention):
+    """E2TTS_Base (upstream F5-TTS `--model E2TTS_Base`): a UNetT backbone (unett.UNetT) with the Vocos vocoder and no
+    duration predictor (pass `duration` to sample(), or estimate it).  Reads a directory holding
+    model_1200000.safetensors and vocab.txt, or a .safetensors / upstream training .pt file (its ema_model_state_dict)
+    with vocab.txt beside it; every key must be one of the model's (unett.checkpoint_state).  "random" builds seeded
+    random E2TTS_Base weights.  There is no FP8 mode, no quantised checkpoint and no BigVGAN for this backbone yet."""
+    import os
+    from .unett import E2_BASE_CONFIG, UNetT, random_unett_weights
+    if fp8 is not None or fp8_attention:
+        raise ValueError("model_version='e2' has no FP8 mode (fp8 / fp8_attention): it runs in bf16")
+    if quantization_bits is not None:
+        raise ValueError("model_version='e2' has no quantised checkpoints (quantization_bits)")
+    if isinstance(vocoder, str) and vocoder != "vocos":
+        raise ValueError(f"model_version='e2' decodes with Vocos only, not vocoder={vocoder!r}")
+    if vocoder == "vocos":
+        vocoder = None
+    cfg = E2_BASE_CONFIG
+
+    def backbone(text_num_embeds: int, dim: int = cfg.dim, depth: int = cfg.depth, ff_mult: int = cfg.ff_mult) -> UNetT:
+        return UNetT(dim=dim, depth=depth, heads=dim // 64, ff_mult=ff_mult, mel_dim=cfg.mel_dim,
+                     text_num_embeds=text_num_embeds, text_dim=cfg.text_dim, text_mask_padding=False, conv_layers=0,
+                     pe_attn_head=cfg.pe_attn_head, skip_connect_type="concat", device=device)
+
+    if hf_model_name_or_path == "random":
+        vp = vocab_path or os.environ.get("F5_VOCAB_PATH")
+        vocab, vocab_source = (read_vocab(Path(vp)), str(vp)) if vp is not None else (ascii_vocab(), "ascii")
+        net = backbone(cfg.text_num_embeds)
+        load_weights_distributed(net, lambda: random_unett_weights(cfg, seed=1234))
+        if vocoder is None:
+            vocoder = Vocos(VocosConfig(), device).load_weights(random_vocos_weights()).decode
+        m = cls(transformer=net, vocab_char_map=vocab, vocoder=vocoder or None)
+        m.vocab_source = vocab_source
+        return m
+
+    given = Path(hf_model_name_or_path)
+    if given.is_file():
+        if given.suffix not in (".safetensors", ".pt"):
+            raise ValueError(f"{given} is not a .safetensors or .pt checkpoint")
+        path, model_file = given.parent, given
+    else:
+        path = _resolve(hf_model_name_or_path, None, "e2")
+        if path is None:
+            raise ValueError(f"Could not find model {hf_model_name_or_path}")
+        model_file = path / MODEL_VERSIONS["e2"][0]
+    vocab = read_vocab(path / "vocab.txt")
+
+    if model_file.suffix == ".pt":
+        ck = torch.load(str(model_file), map_location="cpu", weights_only=True)
+        if "ema_model_state_dict" not in ck:
+            raise ValueError(f"{model_file} has no ema_model_state_dict")
+        sd = {k: v.float() for k, v in ck["ema_model_state_dict"].items()}
+    else:
+        from safetensors.torch import load_file
+        sd = load_file(str(model_file))
+    # width, depth and FF width from the tensors (E2TTS_Base: 1024, 24, 4); the key check then covers every layer
+    sd = {k[len("ema_model."):] if k.startswith("ema_model.") else k: v for k, v in sd.items()}
+    try:
+        dim = sd["transformer.proj_out.weight"].shape[1]
+        depth = 1 + max(int(k.split(".")[2]) for k in sd if k.startswith("transformer.layers."))
+        ff_mult = sd["transformer.layers.0.4.ff.0.0.weight"].shape[0] // dim
+    except (KeyError, ValueError) as e:
+        raise ValueError(f"{model_file} is not an E2TTS_Base-form UNetT checkpoint ({e!r})") from None
+    net = backbone(len(vocab) - 1, dim, depth, ff_mult)
+    load_weights_distributed(net, lambda: sd)
+    if vocoder is None:
+        vpath = _resolve_vocos(path)
+        if vpath is None:
+            raise FileNotFoundError(
+                f"no Vocos checkpoint found (looked for {', '.join(VOCOS_FILES)} in {path}, $F5_VOCOS_PATH and the hub "
+                f"repo {VOCOS_REPO}); pass vocoder=False to get mel spectrograms from sample() instead")
+        from safetensors.torch import load_file
+        vocoder = Vocos(VocosConfig(), device).load_weights(convert_vocos_upstream(load_file(str(vpath)))).decode
+    elif vocoder is False:
+        vocoder = None
+    return cls(transformer=net, vocab_char_map=vocab, vocoder=vocoder)

@@ -99,6 +99,14 @@ typedef struct f5_gemm_args {
   int32_t w_static;       /* nonzero: `w` is never written by work that precedes this call on the stream
                              (model weights): the kernel may start fetching it before its programmatic
                              dependency on the preceding kernel has resolved                           */
+  /* RMSNorm consumer mode (ABI 2.006; the field occupies what was padding after w_static, so sizeof and every other
+   * offset are unchanged): nonzero makes the GEMM consume RMSNorm(x) = x * sqrt(k) / max(||x||_2, 1e-12) * g through
+   * the linearity of the Linear, with g folded into `w` at pack time (w = W diag(g)):
+   *     out = acc * sqrt(k) / max(sqrt(sum_col x^2), 1e-12) + bias,
+   * the row's sum of squares taken from `ln_in_stats` ([rows][k / 64][2], as the fused-AdaLN producer writes them: a
+   * producer with out2_bf16 and ln_stats but no ln_scale writes a plain bf16 copy of x).  Needs ln_in_stats, no ln_tab,
+   * no second output, a plain bf16 GEMM with k % 128 == 0.  An all-zero row gives bias (0 * finite).  0 = off. */
+  int32_t ln_rms;
   const void* prefetch;   /* NULL, or device memory (weights of a later GEMM) to pull into L2       */
   int64_t prefetch_bytes;
   /* Fused AdaLayerNormZero (dit.py:262-271, 281-290; call sites dit.py:313,321,397) by linearity of the Linear that
@@ -404,6 +412,84 @@ int f5_ode_eval_times(const float* h_t_grid, int32_t steps, int32_t method, floa
 int f5_ode_sample(const f5_dit_weights* w, const f5_dit_buffers* b, const float* h_t_grid,
                   int32_t steps, int32_t method, float cfg_strength, float* y, float* trajectory,
                   float* scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------ *
+ * UNetT (ABI 2.006): the flat UNet-Transformer backbone of upstream F5-TTS's E2TTS_Base (f5_tts/model/backbones/unett.py,
+ * skip_connect_type "concat", qk_norm None, conv_layers 0, text_mask_padding False).  Per utterance of N frames:
+ *   t = TimestepEmbedding(time); x = InputEmbedding(x, cond, TextEmbedding(text)) (the DiT's, with a plain embedding
+ *   gather: no position table, no ConvNeXt); x = [t | x], N + 1 rows, the time token at row 0 (RoPE positions 0..N);
+ *   for layer i < depth/2: push x; for i >= depth/2: x = skip_proj_i([x | pop()]) (no residual);
+ *   x += attn(RMSNorm(x)); x += ff(RMSNorm(x)); v = proj_out(RMSNorm_out(x)[1:]).
+ * RMSNorm is x * sqrt(D) / max(||x||, 1e-12) * g; each g is folded into the consuming weight (f5_gemm_args.ln_rms).
+ * Skip slots: bf16 [depth/2][rows, 2D]; slot j's right half is x at the start of layer j (written by the GEMM that
+ * produced it, and read by that layer's QKV with lda = 2D), its left half x at the start of layer depth - 1 - j (written
+ * by the FF2 before it), so skip_proj is one GEMM with k = 2D over the slot.  bf16 + fp32 only (no FP8 modes).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct f5_unett_weights {
+  int32_t dim, depth, heads, ff_inner, mel_dim, text_dim;
+  int32_t text_rows;      /* rows of the embedding table (text_num_embeds + 1) */
+  int32_t ct_ld;          /* padded width of [cond|text] (multiple of 64) */
+  int32_t rope_heads;     /* rotary embedding on the first rope_heads heads of q and k (E2TTS_Base: 1); 0 = all */
+  int32_t reserved;
+  const float* time_w0; const float* time_b0;   /* fp32 [D,256],[D] */
+  const float* time_w2; const float* time_b2;   /* fp32 [D,D],[D] */
+  const float* text_emb;                        /* fp32 [text_rows, text_dim] */
+  const void* in_x_w;                           /* bf16 [D, 128] */
+  const void* in_ct_w;                          /* bf16 [D, ct_ld] */
+  const float* in_b;                            /* fp32 [D] */
+  const void* conv_w[2]; const float* conv_b[2];/* bf16 [D, 31*64], fp32 [D] */
+  /* HOST array [depth]: qkv_w = bf16([Wq; Wk; Wv] diag(attn_norm.g)), ff1_w = bf16(W1 diag(ff_norm.g)), out_w / ff2_w
+   * as in the DiT; every FP8 field NULL */
+  const f5_dit_block_weights* blocks;
+  const void* skip_w;                           /* bf16 [depth/2][D, 2D]: skip_proj of layer depth/2 + i at i */
+  const void* proj_w; const float* proj_b;      /* bf16(W diag(norm_out.g)) [mel_dim, D], fp32 [mel_dim] */
+} f5_unett_weights;
+
+/* Device buffers of one sampling session; R = (cfg ? 2 : 1) * batch * frames rows of frames, R1 = R + (cfg ? 2 : 1) *
+ * batch rows with the time token.  The skip slots cost depth/2 * R1 * 2D * 2 bytes. */
+typedef struct f5_unett_buffers {
+  int32_t batch, frames, cfg, n_times;
+  int32_t text_len_max;       /* nt: columns of `text` */
+  int32_t drop_flags;         /* only when cfg == 0: bit0 drop_audio_cond, bit1 drop_text */
+  /* inputs */
+  const int32_t* text;        /* int32 [batch, nt], pad -1 */
+  const int32_t* seq_len1;    /* int32 [R / frames]: valid frames + 1 (the time row), or NULL when mask is None */
+  const int32_t* valid_len;   /* int32 [R / frames]: frame bucketing as f5_dit_buffers.valid_len, or NULL */
+  const int32_t* valid_len1;  /* int32 [R / frames]: valid_len + 1; set exactly when valid_len is */
+  const float* cond;          /* fp32 [batch, frames, mel_dim] */
+  const float* tvals;         /* fp32 [n_times] */
+  const float* rope;          /* fp32 [frames + 1, 32, 2] */
+  /* precomputed by f5_unett_precompute */
+  float* hoist;               /* fp32 [R, D] */
+  float* t_emb;               /* fp32 [n_times, D] */
+  /* scratch */
+  float* text_x;              /* fp32 [R, text_dim] */
+  void* ct_bf16;              /* bf16 [R, ct_ld] */
+  void* silu_t;               /* bf16 [n_times, D] */
+  void* y_bf16;               /* bf16 [R, 128]: current ODE state */
+  float* h;                   /* fp32 [R, D]: input embedding */
+  float* x;                   /* fp32 [R1, D] residual stream */
+  void* a_bf16;               /* bf16 [R1, D] */
+  void* c_bf16;               /* bf16 [R1, D] */
+  void* qkv_bf16;             /* bf16 [R1, 3D] */
+  void* ff_bf16;              /* bf16 [R1, ff_inner] */
+  float* ln_stats;            /* fp32 [R1, D/64, 2] */
+  void* skip;                 /* bf16 [depth/2, R1, 2D] */
+  float* v;                   /* fp32 [R1, mel_dim]: output rows, the time rows included */
+} f5_unett_buffers;
+
+/* text embedding, hoisted [cond | text] projection, TimestepEmbedding of every evaluation time */
+int f5_unett_precompute(const f5_unett_weights* w, const f5_unett_buffers* b, void* stream);
+/* one UNetT evaluation at tvals[time_index] on the state in b->y_bf16 -> b->v */
+int f5_unett_forward(const f5_unett_weights* w, const f5_unett_buffers* b, int32_t time_index, void* stream);
+/* f5_ode_sample on this backbone: the solver update reads v past each utterance's time row */
+int f5_unett_ode_sample(const f5_unett_weights* w, const f5_unett_buffers* b, const float* h_t_grid, int32_t steps,
+                        int32_t method, float cfg_strength, float* y, float* trajectory, float* scratch, void* stream);
+/* Kernel test entry: the time-token pack.  xe fp32 [batch, frames, D] (the input embedding), t_emb fp32 [D] ->
+ * x fp32 [batch, frames + 1, D] with t_emb at row 0 of each utterance, x_bf16 = bf16(x) [batch * (frames + 1), ld_bf16],
+ * ln_stats fp32 [batch * (frames + 1), D / 64, 2] (sum, sum of squares per 64 columns). */
+int f5_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, int64_t ld_bf16, float* ln_stats,
+                       int32_t batch, int32_t frames, int32_t dim, void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
  * DurationPredictor (duration.py:97-253, inference branch; call site cfm.py:253-262,307-308): runs
