@@ -222,6 +222,7 @@ class F5TTS:
         pad_frames: Optional[int] = None,
         frame_bucket: Optional[int] = None,
         cond_sample_rate: Optional[int] = None,
+        edit_mask: Optional[torch.Tensor] = None,
     ) -> Tuple[torch.Tensor, torch.Tensor]:
         """cfm.py:264-402.  Extensions (default-compatible): `y0` injects the initial noise
         (b, n, mel) — MLX's RNG stream cannot be reproduced, so seeded parity is defined on injected
@@ -231,7 +232,11 @@ class F5TTS:
         because the reference's padding leaks into GRN and the ODE on padded frames; `frame_bucket` (default
         self.frame_bucket) reuses one plan / CUDA graph for all lengths of a bucket, results unchanged;
         `cond_sample_rate` is the rate of a raw-wave `cond` (None: the mel front-end's own rate, 24 kHz) — another rate
-        is resampled on the device (audio.resample, torchaudio's default windowed sinc) before the mel."""
+        is resampled on the device (audio.resample, torchaudio's default windowed sinc) before the mel.
+        `edit_mask` (speech editing, upstream F5-TTS's `CFM.sample(edit_mask=)`): bool [b, n_c], n_c the conditioning's
+        frame count (a raw-wave `cond`: the frames of its mel); False frames are regenerated, True frames condition.
+        The conditioning mask becomes `lens_to_mask(lens) & edit_mask`, with columns past n_c counting as True.  The
+        mask is not part of the plan: an edit reuses the buffers and CUDA graph of any call of the same shape."""
         dev = self.transformer.device
         if method not in METHODS:
             raise ValueError(f"Unknown method: {method}")
@@ -252,6 +257,13 @@ class F5TTS:
             raise ValueError("cond_sample_rate applies to a raw-wave cond [1, t]; this cond is a mel spectrogram")
         cond = cond.to(dev).float()
         batch, cond_seq_len = cond.shape[:2]
+        if edit_mask is not None:
+            if not isinstance(edit_mask, torch.Tensor) or edit_mask.dtype != torch.bool:
+                raise ValueError(f"edit_mask must be a bool tensor, got {getattr(edit_mask, 'dtype', type(edit_mask))}")
+            if tuple(edit_mask.shape) != (batch, cond_seq_len):
+                raise ValueError(f"edit_mask must have shape [batch, conditioning frames] = {(batch, cond_seq_len)}, "
+                                 f"got {tuple(edit_mask.shape)}")
+            edit_mask = edit_mask.detach().cpu()
         if not exists(lens):
             lens = torch.full((batch,), cond_seq_len, dtype=torch.float32)
         lens = lens.detach().cpu().float()
@@ -274,6 +286,10 @@ class F5TTS:
         elif duration is None:
             raise ValueError("Duration must be provided or a duration predictor must be set.")
         cond_mask = lens_to_mask(lens)
+        if edit_mask is not None:
+            w = cond_mask.shape[-1]                                   # max(lens): past n_c when the text is longer
+            em = edit_mask[:, :w]
+            cond_mask = cond_mask & F.pad(em, (0, w - em.shape[-1]), value=True)
         if isinstance(duration, int):
             duration = torch.full((batch,), duration, dtype=torch.float32)
         duration = torch.as_tensor(duration).detach().cpu().float().reshape(-1)

@@ -68,7 +68,7 @@ def sample_sharded(f5, cond: torch.Tensor, text, duration: torch.Tensor, **kw):
     to the rank whose shard_range holds it, every shard pads to the GLOBAL frame count (one int all-reduce — the only
     communication before the host-side gather), and rank 0 receives the mel outputs in global order (others: None).
     `cond` (b, n, mel), `text` (b, nt) int tensor or list of str, `duration` (b,) are the GLOBAL batch on every rank;
-    `y0`, if given, is the global noise (b, N, mel)."""
+    `y0`, if given, is the global noise (b, N, mel); `edit_mask`, if given, the global speech-editing mask (b, n)."""
     rank, ws = world()
     b = cond.shape[0]
     mine = shard_range(b, ws, rank)
@@ -87,8 +87,11 @@ def sample_sharded(f5, cond: torch.Tensor, text, duration: torch.Tensor, **kw):
     lens = torch.maximum(text_len.float(), torch.full((len(mine),), float(cond.shape[1])))
     n_local = int(torch.clip(torch.maximum(lens + 1, duration[sl].float()), 0, kw.get("max_duration", 4096)).max().item())
     n_glob = global_frames(n_local, device=dev)
-    y0 = kw.pop("y0", None)
+    y0, edit_mask = kw.pop("y0", None), kw.pop("edit_mask", None)
     if y0 is not None:
         y0 = y0[sl]
-    out, _ = f5.sample(cond[sl], text_l, duration[sl], y0=y0, pad_frames=n_glob, return_trajectory=False, **kw)
+    if edit_mask is not None:
+        edit_mask = edit_mask[sl]
+    out, _ = f5.sample(cond[sl], text_l, duration[sl], y0=y0, edit_mask=edit_mask, pad_frames=n_glob,
+                       return_trajectory=False, **kw)
     return gather_objects([o.cpu() for o in out])
