@@ -71,6 +71,116 @@ template int text_embedding(const f5_dit_weights*, const f5_dit_buffers*, int, i
 template int text_embedding(const f5_duration_weights*, const f5_duration_buffers*, int, int, int, const int*,
                             const int*, bool, cudaStream_t);
 
+int check_dims(const char* who, int dim, int heads, int mel_dim) {
+  // the implicit grouped conv reads 64-channel blocks, so each of its 16 groups (dim/16 channels) must lie inside one
+  // block: dim/16 divides 64, which within 256..1024 leaves 256, 512 and 1024
+  F5_REQUIRE(dim % 128 == 0 && dim >= 256 && dim <= 1024 && 64 % (dim / 16) == 0,
+             "%s: dim %d unsupported (256, 512 or 1024: the conv's dim/16-channel groups must tile 64-channel blocks)",
+             who, dim);
+  F5_REQUIRE(dim == heads * 64, "%s: dim %d != heads %d * 64", who, dim, heads);
+  F5_REQUIRE(mel_dim % 4 == 0 && mel_dim <= 128, "%s: mel_dim %d", who, mel_dim);
+  return 0;
+}
+
+template <typename Weights, typename Buffers>
+int input_embed_hoist(const Weights* w, const Buffers* b, cudaStream_t st) {
+  const int D = w->dim, N = b->frames, B = b->batch;
+  const int BU = (b->cfg ? 2 : 1) * B;
+  const int R = BU * N;
+  if (int e = launch_concat_cond_text(b->cond, w->mel_dim, B, N, b->text_x, w->text_dim, b->ct_bf16, w->ct_ld, R,
+                                      b->cfg ? B * N : ((b->drop_flags & 1) ? 0 : R), st))
+    return e;
+  f5_gemm_args g = gemm_args(b->ct_bf16, w->ct_ld, w->in_ct_w, w->ct_ld, R, D, w->ct_ld, b->hoist, D, false, true);
+  g.bias = w->in_b;
+  if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }   // bucket rows stay 0
+  return f5_gemm_bf16(&g, st);
+}
+template int input_embed_hoist(const f5_unett_weights*, const f5_unett_buffers*, cudaStream_t);
+
+template <typename Weights, typename Buffers>
+int input_embedding(const Weights* w, const Buffers* b, void* out, cudaStream_t st, f5_gemm_args* conv2) {
+  const int D = w->dim, N = b->frames;
+  const int BU = (b->cfg ? 2 : 1) * b->batch;
+  const int R = BU * N;
+  {
+    f5_gemm_args g = gemm_args(b->y_bf16, 128, w->in_x_w, 128, R, D, 128, b->h, D, false, true);
+    g.resid = b->hoist; g.ldr = D;
+    g.out2_bf16 = b->a_bf16; g.ldo2 = D;
+    // bucket rows (>= valid_len): x·Wx masked to 0 + hoist (0 there) = 0 — the conv below sees the reference's zero padding
+    if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }
+    if (int e = f5_gemm_bf16(&g, st)) return e;
+  }
+  {
+    f5_gemm_args g = conv_pos_args(b->a_bf16, w->conv_w[0], w->conv_b[0], b->c_bf16, true, D, N, BU, true);
+    g.row_len = b->valid_len;      // NULL, or: the second conv's input is zero on bucket rows too
+    if (int e = f5_gemm_bf16(&g, st)) return e;
+  }
+  *conv2 = conv_pos_args(b->c_bf16, w->conv_w[1], w->conv_b[1], out, false, D, N, BU, true);
+  conv2->resid = b->h; conv2->ldr = D;
+  return 0;
+}
+template int input_embedding(const f5_unett_weights*, const f5_unett_buffers*, void*, cudaStream_t, f5_gemm_args*);
+
+template <typename Weights, typename Buffers>
+int ode_sample(int (*forward)(const Weights*, const Buffers*, int32_t, void*), const Weights* w, const Buffers* b,
+               OdeUpdateParams u, const char* who, const float* t, int steps, int method, float cfg_strength, float* y,
+               float* trajectory, float* scratch, cudaStream_t st) {
+  F5_REQUIRE(t && steps >= 2 && y, "%s: bad arguments", who);
+  F5_REQUIRE(method >= 0 && method <= 2, "%s: unknown method %d", who, method);
+  F5_REQUIRE((cfg_strength >= 1e-5f) == (b->cfg != 0), "%s: buffers built with cfg=%d but cfg_strength=%g", who,
+             b->cfg, cfg_strength);
+  const int per = method == 0 ? 1 : (method == 1 ? 2 : 4);
+  F5_REQUIRE(b->n_times == (steps - 1) * per, "%s: n_times %d != %d", who, b->n_times, (steps - 1) * per);
+  F5_REQUIRE(method == 0 || scratch, "%s: scratch required for midpoint/rk4", who);
+  const int BN = b->batch * b->frames, d = w->mel_dim;
+  const size_t state = (size_t)BN * d;
+  const long long dup = b->cfg ? BN : 0;
+
+  // A operand of the first x-projection: bf16(y0), both CFG halves
+  const float* y_cur = trajectory ? trajectory : y;
+  if (int e = launch_cast_pad_bf16(y_cur, d, b->y_bf16, 128, BN, dup, st)) return e;
+
+  u.ldv = d; u.cfg_strength = cfg_strength;
+  u.y_bf16 = reinterpret_cast<__nv_bfloat16*>(b->y_bf16); u.ld_bf16 = 128;
+  u.bf16_copy_row_offset = dup;
+  u.rows = BN; u.d = d;
+  float* y_tmp = scratch;
+  float* k_acc = scratch ? scratch + state : nullptr;
+
+  int ti = 0;
+  for (int i = 0; i + 1 < steps; ++i) {
+    const float dt = t[i + 1] - t[i];
+    float* y_next = trajectory ? trajectory + (size_t)(i + 1) * state : y;
+    u.y_base = y_cur;
+    if (method == 0) {
+      if (int e = forward(w, b, ti++, st)) return e;
+      u.y_out = y_next; u.a = dt; u.k_acc = nullptr; u.use_acc = 0;
+      if (int e = launch_ode_update(u, st)) return e;
+    } else if (method == 1) {
+      if (int e = forward(w, b, ti++, st)) return e;
+      u.y_out = y_tmp; u.a = 0.5f * dt; u.k_acc = nullptr; u.use_acc = 0;
+      if (int e = launch_ode_update(u, st)) return e;
+      if (int e = forward(w, b, ti++, st)) return e;
+      u.y_out = y_next; u.a = dt;
+      if (int e = launch_ode_update(u, st)) return e;
+    } else {
+      const float as[4] = {0.5f * dt, 0.5f * dt, dt, dt / 6.f};
+      const float ws[4] = {1.f, 2.f, 2.f, 1.f};
+      for (int s = 0; s < 4; ++s) {
+        if (int e = forward(w, b, ti++, st)) return e;
+        u.k_acc = k_acc; u.acc_w = ws[s]; u.acc_init = (s == 0); u.use_acc = (s == 3);
+        u.y_out = (s == 3) ? y_next : y_tmp; u.a = as[s];
+        if (int e = launch_ode_update(u, st)) return e;
+      }
+    }
+    y_cur = y_next;
+  }
+  return 0;
+}
+template int ode_sample(int (*)(const f5_unett_weights*, const f5_unett_buffers*, int32_t, void*),
+                        const f5_unett_weights*, const f5_unett_buffers*, OdeUpdateParams, const char*, const float*,
+                        int, int, float, float*, float*, float*, cudaStream_t);
+
 // What f5_dit_forward runs, chosen by the buffers the caller binds (see f5_dit_buffers in include/f5_b200.h)
 struct DitMode {
   bool fused;   // AdaLN LayerNorm folded into the GEMM epilogues (ln_stats / ln_tab / ln_prep)
@@ -133,13 +243,7 @@ static int check_mode(const f5_dit_weights* w, const f5_dit_buffers* b, DitMode&
 
 static int check_common(const f5_dit_weights* w, const f5_dit_buffers* b, DitMode& mode) {
   F5_REQUIRE(w && b, "dit: null weights/buffers");
-  // the implicit grouped conv reads 64-channel blocks, so each of its 16 groups (dim/16 channels) must lie inside one
-  // block: dim/16 divides 64, which within 256..1024 leaves 256, 512 and 1024
-  F5_REQUIRE(w->dim % 128 == 0 && w->dim >= 256 && w->dim <= 1024 && 64 % (w->dim / 16) == 0,
-             "dit: dim %d unsupported (256, 512 or 1024: the conv's dim/16-channel groups must tile 64-channel blocks)",
-             w->dim);
-  F5_REQUIRE(w->dim == w->heads * 64, "dit: dim %d != heads %d * 64", w->dim, w->heads);
-  F5_REQUIRE(w->mel_dim % 4 == 0 && w->mel_dim <= 128, "dit: mel_dim %d", w->mel_dim);
+  if (int e = check_dims("dit", w->dim, w->heads, w->mel_dim)) return e;
   F5_REQUIRE(w->blocks && w->depth > 0, "dit: no blocks");
   F5_REQUIRE(b->batch > 0 && b->frames > 0 && b->n_times > 0, "dit: bad buffer shape");
   F5_REQUIRE(w->text_unmasked == 0 || w->text_unmasked == 1, "dit: text_unmasked %d is not 0 or 1", w->text_unmasked);
@@ -258,10 +362,8 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
   DitMode mode;
   if (int e = check_common(w, b, mode)) return e;
   cudaStream_t st = (cudaStream_t)stream_;
-  const int D = w->dim, N = b->frames, B = b->batch;
+  const int D = w->dim, B = b->batch;
   const int BU = (b->cfg ? 2 : 1) * B;  // row-utterances
-  const int R = BU * N;
-  const int C = w->text_dim;
 
   // ---- TextEmbedding (dit.py:196-229) for the cond rows and, with CFG, the text-dropped rows ----
   // Unmasked text (mask_padding=False, dit.py:226-227): filler rows keep embed[0] + position through every ConvNeXt
@@ -273,15 +375,7 @@ extern "C" int f5_dit_precompute(const f5_dit_weights* w, const f5_dit_buffers* 
     return e;
 
   // ---- hoisted part of InputEmbedding.proj (dit.py:248-249): [cond | text] · W[:,100:]^T + b ----
-  if (int e = launch_concat_cond_text(b->cond, w->mel_dim, B, N, b->text_x, C, b->ct_bf16, w->ct_ld,
-                                      R, b->cfg ? B * N : ((b->drop_flags & 1) ? 0 : R), st))
-    return e;
-  {
-    f5_gemm_args g = gemm_args(b->ct_bf16, w->ct_ld, w->in_ct_w, w->ct_ld, R, D, w->ct_ld, b->hoist, D, false, true);
-    g.bias = w->in_b;
-    if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }   // bucket rows stay 0
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
+  if (int e = input_embed_hoist(w, b, st)) return e;
 
   // ---- TimestepEmbedding for every evaluation time, then ALL AdaLN linears as one GEMM ----
   if (int e = launch_time_mlp(b->tvals, b->n_times, D, w->time_w0, w->time_b0, w->time_w2,
@@ -332,21 +426,8 @@ extern "C" int f5_dit_forward(const f5_dit_weights* w, const f5_dit_buffers* b, 
 
   // ---- InputEmbedding (dit.py:249-251): x·Wx + hoist, then + ConvPositionEmbedding ----
   {
-    f5_gemm_args g = gemm_args(b->y_bf16, 128, w->in_x_w, 128, R, D, 128, b->h, D, false, true);
-    g.resid = b->hoist; g.ldr = D;
-    g.out2_bf16 = b->a_bf16; g.ldo2 = D;
-    // bucket rows (>= valid_len): x·Wx masked to 0 + hoist (0 there) = 0 — the conv below sees the reference's zero padding
-    if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
-  {
-    f5_gemm_args g = conv_pos_args(b->a_bf16, w->conv_w[0], w->conv_b[0], b->c_bf16, true, D, N, BU, true);
-    g.row_len = b->valid_len;      // NULL, or: the second conv's input is zero on bucket rows too
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
-  {
-    f5_gemm_args g = conv_pos_args(b->c_bf16, w->conv_w[1], w->conv_b[1], b->x, false, D, N, BU, true);
-    g.resid = b->h; g.ldr = D;
+    f5_gemm_args g;
+    if (int e = input_embedding(w, b, b->x, st, &g)) return e;
     ln_producer(g, mode, b, D, mod + D, mode.fp8);   // the stream's first producer: block 0's attn_norm
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
@@ -446,59 +527,8 @@ extern "C" int f5_ode_sample(const f5_dit_weights* w, const f5_dit_buffers* b, c
   if (int e = device_check()) return e;
   DitMode mode;
   if (int e = check_common(w, b, mode)) return e;
-  F5_REQUIRE(t && steps >= 2 && y, "ode_sample: bad arguments");
-  F5_REQUIRE(method >= 0 && method <= 2, "ode_sample: unknown method %d", method);
-  F5_REQUIRE((cfg_strength >= 1e-5f) == (b->cfg != 0),
-             "ode_sample: buffers built with cfg=%d but cfg_strength=%g", b->cfg, cfg_strength);
-  const int per = method == 0 ? 1 : (method == 1 ? 2 : 4);
-  F5_REQUIRE(b->n_times == (steps - 1) * per, "ode_sample: n_times %d != %d", b->n_times,
-             (steps - 1) * per);
-  F5_REQUIRE(method == 0 || scratch, "ode_sample: scratch required for midpoint/rk4");
-  cudaStream_t st = (cudaStream_t)stream_;
-  const int BN = b->batch * b->frames, d = w->mel_dim;
-  const size_t state = (size_t)BN * d;
-  const long long dup = b->cfg ? BN : 0;
-
-  // A operand of the first x-projection: bf16(y0), both CFG halves
-  const float* y_cur = trajectory ? trajectory : y;
-  if (int e = launch_cast_pad_bf16(y_cur, d, b->y_bf16, 128, BN, dup, st)) return e;
-
-  OdeUpdateParams u;
-  memset(&u, 0, sizeof(u));
-  u.v = b->v; u.ldv = d; u.null_row_offset = dup; u.cfg_strength = cfg_strength;
-  u.y_bf16 = reinterpret_cast<__nv_bfloat16*>(b->y_bf16); u.ld_bf16 = 128;
-  u.bf16_copy_row_offset = dup;
-  u.rows = BN; u.d = d;
-  float* y_tmp = scratch;
-  float* k_acc = scratch ? scratch + state : nullptr;
-
-  int ti = 0;
-  for (int i = 0; i + 1 < steps; ++i) {
-    const float dt = t[i + 1] - t[i];
-    float* y_next = trajectory ? trajectory + (size_t)(i + 1) * state : y;
-    u.y_base = y_cur;
-    if (method == 0) {
-      if (int e = f5_dit_forward(w, b, ti++, st)) return e;
-      u.y_out = y_next; u.a = dt; u.k_acc = nullptr; u.use_acc = 0;
-      if (int e = launch_ode_update(u, st)) return e;
-    } else if (method == 1) {
-      if (int e = f5_dit_forward(w, b, ti++, st)) return e;
-      u.y_out = y_tmp; u.a = 0.5f * dt; u.k_acc = nullptr; u.use_acc = 0;
-      if (int e = launch_ode_update(u, st)) return e;
-      if (int e = f5_dit_forward(w, b, ti++, st)) return e;
-      u.y_out = y_next; u.a = dt;
-      if (int e = launch_ode_update(u, st)) return e;
-    } else {
-      const float as[4] = {0.5f * dt, 0.5f * dt, dt, dt / 6.f};
-      const float ws[4] = {1.f, 2.f, 2.f, 1.f};
-      for (int s = 0; s < 4; ++s) {
-        if (int e = f5_dit_forward(w, b, ti++, st)) return e;
-        u.k_acc = k_acc; u.acc_w = ws[s]; u.acc_init = (s == 0); u.use_acc = (s == 3);
-        u.y_out = (s == 3) ? y_next : y_tmp; u.a = as[s];
-        if (int e = launch_ode_update(u, st)) return e;
-      }
-    }
-    y_cur = y_next;
-  }
-  return 0;
+  OdeUpdateParams u = {};
+  u.v = b->v; u.null_row_offset = b->cfg ? (long long)b->batch * b->frames : 0;
+  return ode_sample(f5_dit_forward, w, b, u, "ode_sample", t, steps, method, cfg_strength, y, trajectory, scratch,
+                    (cudaStream_t)stream_);
 }

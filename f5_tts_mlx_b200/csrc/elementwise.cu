@@ -153,6 +153,43 @@ int launch_duration_head(const float* x, int B, int N, int D, const int* len, co
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// UNetT time token (unett.py: x = cat([t[:, None], x], dim=1)): xe fp32 [BU, N, D] -> x fp32 [BU, N + 1, D] with t_emb
+// [D] at row 0 of each utterance, its bf16 copy (row stride ld2) and the per-64-column (sum, sum of squares) of every
+// row, the statistics the GEMM epilogue's producer side writes.  One block per output row, one warp per 64-column unit
+// (two columns per lane).
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+unett_time_pack_kernel(const float* __restrict__ xe, const float* __restrict__ t_emb, float* __restrict__ x,
+                       __nv_bfloat16* __restrict__ xb, long long ld2, float2* __restrict__ ln_stats, int N, int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int n = blockIdx.x, bu = blockIdx.y;     // n: row inside the utterance, 0 = the time token
+  const size_t row = (size_t)bu * (N + 1) + n;
+  const float* src = n == 0 ? t_emb : xe + ((size_t)bu * N + n - 1) * D;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int u = warp; u < D / 64; u += blockDim.x >> 5) {
+    const int c = u * 64 + 2 * lane;
+    const float2 v = *reinterpret_cast<const float2*>(src + c);
+    *reinterpret_cast<float2*>(x + row * D + c) = v;
+    *reinterpret_cast<uint32_t*>(xb + row * ld2 + c) = pack_bf16x2(v.x, v.y);
+    const float s1 = warp_sum(v.x + v.y), s2 = warp_sum(fmaf(v.x, v.x, v.y * v.y));
+    if (lane == 0) ln_stats[row * (D / 64) + u] = make_float2(s1, s2);
+  }
+}
+
+int launch_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, long long ld_bf16,
+                           float* ln_stats, int BU, int N, int D, cudaStream_t st) {
+  ProfScope ps(PROF_OTHER, 0.0, 0.0);
+  F5_REQUIRE(xe && t_emb && x && x_bf16 && ln_stats, "unett_time_pack: null pointer");
+  F5_REQUIRE(BU > 0 && N > 0 && D > 0 && D % 64 == 0 && ld_bf16 >= D && ld_bf16 % 2 == 0,
+             "unett_time_pack: bad shape BU=%d N=%d D=%d ld=%lld", BU, N, D, ld_bf16);
+  F5_CHECK_CUDA(launch_kernel(unett_time_pack_kernel, dim3(N + 1, BU), dim3(128), 0, st, xe, t_emb, x,
+                              reinterpret_cast<__nv_bfloat16*>(x_bf16), ld_bf16, reinterpret_cast<float2*>(ln_stats), N, D));
+  F5_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace f5
 
 extern "C" {
@@ -180,7 +217,7 @@ int f5_grn(const void* h_bf16, void* y_bf16, float* nx_scratch, const float* gam
                         (cudaStream_t)stream);
 }
 
-// ---- kernel test entries: each runs one launcher of the DiT / duration / Vocos paths alone ----
+// ---- kernel test entries: each runs one launcher of the DiT / UNetT / duration / Vocos paths alone ----
 
 int f5_ln_affine_f32(const float* x, float* y, int32_t rows, int32_t dim, const float* w, const float* b,
                      void* stream) {
@@ -254,6 +291,12 @@ int f5_grn_valid(const void* h_bf16, void* y_bf16, float* nx_scratch, const floa
   if (int e = f5::device_check()) return e;
   return f5::launch_grn(h_bf16, y_bf16, nx_scratch, gamma, beta, batch, frames, channels,
                         (cudaStream_t)stream, valid_len);
+}
+
+int f5_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, int64_t ld_bf16, float* ln_stats,
+                       int32_t batch, int32_t frames, int32_t dim, void* stream) {
+  if (int e = f5::device_check()) return e;
+  return f5::launch_unett_time_pack(xe, t_emb, x, x_bf16, ld_bf16, ln_stats, batch, frames, dim, (cudaStream_t)stream);
 }
 
 }  // extern "C"

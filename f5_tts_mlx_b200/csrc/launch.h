@@ -44,8 +44,12 @@ int launch_concat_cond_text(const float* cond, int dc, int Bc, int N, const floa
 int launch_ln_tab_prep(const float* mod, void* prep_bf16, int T, int L, int D, int NM, cudaStream_t st);
 int launch_duration_head(const float* x, int B, int N, int D, const int* len, const float* norm_w,
                          const float* pred_w, float* out, cudaStream_t st);
+// the UNetT time token: x [BU, N + 1, D] = [t_emb | xe] per utterance, its bf16 copy (row stride ld_bf16) and the
+// per-64-column row statistics (f5_unett_time_pack)
+int launch_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, long long ld_bf16,
+                           float* ln_stats, int BU, int N, int D, cudaStream_t st);
 
-// ---- host-side stages shared by the DiT (dit.cu, where they are defined) and the duration predictor ----
+// ---- host-side stages shared by the DiT (dit.cu, where they are defined), the UNetT and the duration predictor ----
 // f5_gemm_args of out = A·W^T with every optional field off; w_static as f5_gemm_args.w_static
 f5_gemm_args gemm_args(const void* a, int64_t lda, const void* w, int64_t ldw, int m, int n, int k, void* out,
                        int64_t ldo, bool out_bf16, bool w_static);
@@ -60,4 +64,22 @@ f5_gemm_args conv_pos_args(const void* a, const void* w, const float* bias, void
 template <typename Weights, typename Buffers>
 int text_embedding(const Weights* w, const Buffers* b, int batch_out, int drop_from, int mask_padding,
                    const int* valid_len, const int* row_len, bool w_static, cudaStream_t st);
+// the dim / heads / mel_dim rules of a backbone, refused with messages beginning `who: `
+int check_dims(const char* who, int dim, int heads, int mel_dim);
+// The rest take f5_dit_* or f5_unett_* weights and buffers.
+// The hoisted part of InputEmbedding.proj (dit.py:248-249): [cond | text] · W[:, mel:]^T + b into b->hoist, from
+// b->cond and the text embedding in b->text_x (audio condition dropped from batch on with CFG, or by drop_flags bit 0)
+template <typename Weights, typename Buffers>
+int input_embed_hoist(const Weights* w, const Buffers* b, cudaStream_t st);
+// InputEmbedding (dit.py:249-251) on the ODE state in b->y_bf16: launches x·Wx + hoist into b->h (bf16 copy in
+// b->a_bf16) and ConvPositionEmbedding's first conv into b->c_bf16, and sets *conv2 to its second conv, fp32 into
+// `out` with residual b->h, for the caller to finish and launch
+template <typename Weights, typename Buffers>
+int input_embedding(const Weights* w, const Buffers* b, void* out, cudaStream_t st, f5_gemm_args* conv2);
+// The fixed-grid solve of f5_ode_sample (Euler, midpoint, RK4) with `forward` as the flow field.  `u` holds the
+// caller's v, v_frames and null_row_offset; the argument checks' messages begin `who: `.
+template <typename Weights, typename Buffers>
+int ode_sample(int (*forward)(const Weights*, const Buffers*, int32_t, void*), const Weights* w, const Buffers* b,
+               OdeUpdateParams u, const char* who, const float* t, int steps, int method, float cfg_strength, float* y,
+               float* trajectory, float* scratch, cudaStream_t st);
 }  // namespace f5

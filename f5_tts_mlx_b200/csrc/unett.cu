@@ -1,73 +1,21 @@
 // UNetT forward (upstream F5-TTS E2TTS_Base) and its ODE loop as a stream-ordered sequence of the sm_90a kernels in
-// this directory, plus the one kernel only this backbone needs, the time-token pack (C-ABI: f5_unett_precompute /
-// f5_unett_forward / f5_unett_ode_sample / f5_unett_time_pack; see include/f5_b200.h).
+// this directory (C-ABI: f5_unett_precompute / f5_unett_forward / f5_unett_ode_sample; see include/f5_b200.h).  Like
+// dit.cu it holds no kernels; the time-token pack, the one kernel only this backbone needs, is in elementwise.cu.
 //
 // Row layout: the frames of an utterance are R = BU * N rows up to the end of the input embedding; the time token then
 // makes every utterance N + 1 rows (R1 = BU * (N + 1)), the time row first.  Each RMSNorm is folded: its gain into the
 // consuming weight at pack time, its row scale sqrt(D) / max(||x||, 1e-12) into the consuming GEMM's epilogue
 // (f5_gemm_args.ln_rms) from the (sum, sum of squares) statistics the producing GEMM writes next to a bf16 copy of x.
-#include <string.h>
-
 #include "host_common.h"
 #include "launch.h"
-#include "ptx.cuh"
 
 namespace f5 {
 namespace {
 
-__device__ __forceinline__ float warp_sum32(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-// ---------------------------------------------------------------------------------------------
-// UNetT time token (unett.py: x = cat([t[:, None], x], dim=1)): xe fp32 [BU, N, D] -> x fp32 [BU, N + 1, D] with t_emb
-// [D] at row 0 of each utterance, its bf16 copy (row stride ld2) and the per-64-column (sum, sum of squares) of every
-// row, the statistics the GEMM epilogue's producer side writes.  One block per output row, one warp per 64-column unit
-// (two columns per lane).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-unett_time_pack_kernel(const float* __restrict__ xe, const float* __restrict__ t_emb, float* __restrict__ x,
-                       __nv_bfloat16* __restrict__ xb, long long ld2, float2* __restrict__ ln_stats, int N, int D) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int n = blockIdx.x, bu = blockIdx.y;     // n: row inside the utterance, 0 = the time token
-  const size_t row = (size_t)bu * (N + 1) + n;
-  const float* src = n == 0 ? t_emb : xe + ((size_t)bu * N + n - 1) * D;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int u = warp; u < D / 64; u += blockDim.x >> 5) {
-    const int c = u * 64 + 2 * lane;
-    const float2 v = *reinterpret_cast<const float2*>(src + c);
-    *reinterpret_cast<float2*>(x + row * D + c) = v;
-    *reinterpret_cast<uint32_t*>(xb + row * ld2 + c) = pack_bf16x2(v.x, v.y);
-    const float s1 = warp_sum32(v.x + v.y), s2 = warp_sum32(fmaf(v.x, v.x, v.y * v.y));
-    if (lane == 0) ln_stats[row * (D / 64) + u] = make_float2(s1, s2);
-  }
-}
-
-int launch_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, long long ld_bf16,
-                           float* ln_stats, int BU, int N, int D, cudaStream_t st) {
-  ProfScope ps(PROF_OTHER, 0.0, 0.0);
-  F5_REQUIRE(xe && t_emb && x && x_bf16 && ln_stats, "unett_time_pack: null pointer");
-  F5_REQUIRE(BU > 0 && N > 0 && D > 0 && D % 64 == 0 && ld_bf16 >= D && ld_bf16 % 2 == 0,
-             "unett_time_pack: bad shape BU=%d N=%d D=%d ld=%lld", BU, N, D, ld_bf16);
-  F5_CHECK_CUDA(launch_kernel(unett_time_pack_kernel, dim3(N + 1, BU), dim3(128), 0, st, xe, t_emb, x,
-                              reinterpret_cast<__nv_bfloat16*>(x_bf16), ld_bf16, reinterpret_cast<float2*>(ln_stats), N, D));
-  F5_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-
-
 int check_unett(const f5_unett_weights* w, const f5_unett_buffers* b) {
   F5_REQUIRE(w && b, "unett: null weights/buffers");
-  F5_REQUIRE(w->dim % 128 == 0 && w->dim >= 256 && w->dim <= 1024 && 64 % (w->dim / 16) == 0,
-             "unett: dim %d unsupported (256, 512 or 1024: the conv's dim/16-channel groups must tile 64-channel blocks)",
-             w->dim);
-  F5_REQUIRE(w->dim == w->heads * 64, "unett: dim %d != heads %d * 64", w->dim, w->heads);
+  if (int e = check_dims("unett", w->dim, w->heads, w->mel_dim)) return e;
   F5_REQUIRE(w->depth > 0 && w->depth % 2 == 0, "unett: depth %d must be even and positive", w->depth);
-  F5_REQUIRE(w->mel_dim % 4 == 0 && w->mel_dim <= 128, "unett: mel_dim %d", w->mel_dim);
   F5_REQUIRE(w->text_dim % 4 == 0 && w->ct_ld % 64 == 0 && w->ct_ld >= w->mel_dim + w->text_dim,
              "unett: text_dim %d / ct_ld %d", w->text_dim, w->ct_ld);
   F5_REQUIRE(w->ff_inner % 64 == 0, "unett: ff_inner %d", w->ff_inner);
@@ -112,12 +60,6 @@ void rms_consumer(f5_gemm_args& g, const float* ln_stats) {
 
 using namespace f5;
 
-extern "C" int f5_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, int64_t ld_bf16,
-                                  float* ln_stats, int32_t batch, int32_t frames, int32_t dim, void* stream) {
-  if (int e = device_check()) return e;
-  return launch_unett_time_pack(xe, t_emb, x, x_bf16, ld_bf16, ln_stats, batch, frames, dim, (cudaStream_t)stream);
-}
-
 extern "C" int f5_unett_precompute(const f5_unett_weights* w, const f5_unett_buffers* b, void* stream_) {
   if (int e = device_check()) return e;
   if (int e = check_unett(w, b)) return e;
@@ -126,7 +68,6 @@ extern "C" int f5_unett_precompute(const f5_unett_weights* w, const f5_unett_buf
   cudaStream_t st = (cudaStream_t)stream_;
   const int D = w->dim, N = b->frames, B = b->batch;
   const int BU = (b->cfg ? 2 : 1) * B;
-  const int R = BU * N;
   // TextEmbedding with conv_layers = 0 and mask_padding = False: the embedding gather alone, filler rows embed[0];
   // bucket rows (>= valid_len) zero.  CFG: the second half text-dropped.
   const int drop_from = b->cfg ? B : ((b->drop_flags & 2) ? 0 : BU);
@@ -134,15 +75,7 @@ extern "C" int f5_unett_precompute(const f5_unett_weights* w, const f5_unett_buf
                                        BU, drop_from, st, 0, b->valid_len))
     return e;
   // hoisted part of InputEmbedding.proj: [cond | text] · W[:, mel:]^T + b
-  if (int e = launch_concat_cond_text(b->cond, w->mel_dim, B, N, b->text_x, w->text_dim, b->ct_bf16, w->ct_ld, R,
-                                      b->cfg ? B * N : ((b->drop_flags & 1) ? 0 : R), st))
-    return e;
-  {
-    f5_gemm_args g = gemm_args(b->ct_bf16, w->ct_ld, w->in_ct_w, w->ct_ld, R, D, w->ct_ld, b->hoist, D, false, true);
-    g.bias = w->in_b;
-    if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }   // bucket rows stay 0
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
+  if (int e = input_embed_hoist(w, b, st)) return e;
   // TimestepEmbedding of every evaluation time: the time tokens
   return launch_time_mlp(b->tvals, b->n_times, D, w->time_w0, w->time_b0, w->time_w2, w->time_b2, b->t_emb, b->silu_t,
                          st);
@@ -155,7 +88,7 @@ extern "C" int f5_unett_forward(const f5_unett_weights* w, const f5_unett_buffer
   cudaStream_t st = (cudaStream_t)stream_;
   const int D = w->dim, N = b->frames, N1 = N + 1, F = w->ff_inner, H = w->depth / 2;
   const int BU = (b->cfg ? 2 : 1) * b->batch;
-  const int R = BU * N, R1 = BU * N1;
+  const int R1 = BU * N1;
   const bool prefetch = R1 <= 16384;   // as the DiT: weights prefetched into L2 while they are comparable to activations
   __nv_bfloat16* skip = reinterpret_cast<__nv_bfloat16*>(b->skip);
   auto slot = [&](int j) { return skip + (size_t)j * R1 * 2 * D; };
@@ -165,20 +98,8 @@ extern "C" int f5_unett_forward(const f5_unett_weights* w, const f5_unett_buffer
 
   // ---- InputEmbedding: x·Wx + hoist, then + ConvPositionEmbedding (the DiT's, on R rows) ----
   {
-    f5_gemm_args g = gemm_args(b->y_bf16, 128, w->in_x_w, 128, R, D, 128, b->h, D, false, true);
-    g.resid = b->hoist; g.ldr = D;
-    g.out2_bf16 = b->a_bf16; g.ldo2 = D;
-    if (b->valid_len) { g.rows_per_batch = N; g.num_batches = BU; g.row_len = b->valid_len; }
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
-  {
-    f5_gemm_args g = conv_pos_args(b->a_bf16, w->conv_w[0], w->conv_b[0], b->c_bf16, true, D, N, BU, true);
-    g.row_len = b->valid_len;
-    if (int e = f5_gemm_bf16(&g, st)) return e;
-  }
-  {
-    f5_gemm_args g = conv_pos_args(b->c_bf16, w->conv_w[1], w->conv_b[1], b->h, false, D, N, BU, true);
-    g.resid = b->h; g.ldr = D;
+    f5_gemm_args g;
+    if (int e = input_embedding(w, b, b->h, st, &g)) return e;
     if (int e = f5_gemm_bf16(&g, st)) return e;
   }
   // ---- time token at row 0: x [BU, N + 1, D], its bf16 copy in the right half of skip slot 0 (layer 0's push and its
@@ -258,60 +179,10 @@ extern "C" int f5_unett_ode_sample(const f5_unett_weights* w, const f5_unett_buf
                                    void* stream_) {
   if (int e = device_check()) return e;
   if (int e = check_unett(w, b)) return e;
-  F5_REQUIRE(t && steps >= 2 && y, "unett_ode_sample: bad arguments");
-  F5_REQUIRE(method >= 0 && method <= 2, "unett_ode_sample: unknown method %d", method);
-  F5_REQUIRE((cfg_strength >= 1e-5f) == (b->cfg != 0),
-             "unett_ode_sample: buffers built with cfg=%d but cfg_strength=%g", b->cfg, cfg_strength);
-  const int per = method == 0 ? 1 : (method == 1 ? 2 : 4);
-  F5_REQUIRE(b->n_times == (steps - 1) * per, "unett_ode_sample: n_times %d != %d", b->n_times, (steps - 1) * per);
-  F5_REQUIRE(method == 0 || scratch, "unett_ode_sample: scratch required for midpoint/rk4");
-  cudaStream_t st = (cudaStream_t)stream_;
-  const int BN = b->batch * b->frames, d = w->mel_dim;
-  const size_t state = (size_t)BN * d;
-  const long long dup = b->cfg ? BN : 0;
-
-  const float* y_cur = trajectory ? trajectory : y;
-  if (int e = launch_cast_pad_bf16(y_cur, d, b->y_bf16, 128, BN, dup, st)) return e;
-
-  OdeUpdateParams u;
-  memset(&u, 0, sizeof(u));
   // v: frames + 1 rows per utterance (time row first); the null (CFG) rows start after batch of them
-  u.v = b->v; u.ldv = d; u.v_frames = b->frames;
+  OdeUpdateParams u = {};
+  u.v = b->v; u.v_frames = b->frames;
   u.null_row_offset = b->cfg ? (long long)b->batch * (b->frames + 1) : 0;
-  u.cfg_strength = cfg_strength;
-  u.y_bf16 = reinterpret_cast<__nv_bfloat16*>(b->y_bf16); u.ld_bf16 = 128;
-  u.bf16_copy_row_offset = dup;
-  u.rows = BN; u.d = d;
-  float* y_tmp = scratch;
-  float* k_acc = scratch ? scratch + state : nullptr;
-
-  int ti = 0;
-  for (int i = 0; i + 1 < steps; ++i) {
-    const float dt = t[i + 1] - t[i];
-    float* y_next = trajectory ? trajectory + (size_t)(i + 1) * state : y;
-    u.y_base = y_cur;
-    if (method == 0) {
-      if (int e = f5_unett_forward(w, b, ti++, st)) return e;
-      u.y_out = y_next; u.a = dt; u.k_acc = nullptr; u.use_acc = 0;
-      if (int e = launch_ode_update(u, st)) return e;
-    } else if (method == 1) {
-      if (int e = f5_unett_forward(w, b, ti++, st)) return e;
-      u.y_out = y_tmp; u.a = 0.5f * dt; u.k_acc = nullptr; u.use_acc = 0;
-      if (int e = launch_ode_update(u, st)) return e;
-      if (int e = f5_unett_forward(w, b, ti++, st)) return e;
-      u.y_out = y_next; u.a = dt;
-      if (int e = launch_ode_update(u, st)) return e;
-    } else {
-      const float as[4] = {0.5f * dt, 0.5f * dt, dt, dt / 6.f};
-      const float ws[4] = {1.f, 2.f, 2.f, 1.f};
-      for (int s = 0; s < 4; ++s) {
-        if (int e = f5_unett_forward(w, b, ti++, st)) return e;
-        u.k_acc = k_acc; u.acc_w = ws[s]; u.acc_init = (s == 0); u.use_acc = (s == 3);
-        u.y_out = (s == 3) ? y_next : y_tmp; u.a = as[s];
-        if (int e = launch_ode_update(u, st)) return e;
-      }
-    }
-    y_cur = y_next;
-  }
-  return 0;
+  return ode_sample(f5_unett_forward, w, b, u, "unett_ode_sample", t, steps, method, cfg_strength, y, trajectory,
+                    scratch, (cudaStream_t)stream_);
 }

@@ -150,8 +150,134 @@ def _check_prefix_padding(text: torch.Tensor) -> None:
         raise ValueError("text ids must be right-padded with -1 (interior -1 is not supported)")
 
 
-class DiT:
+def _stream() -> C.c_void_p:
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+class Backbone:
+    """What the DiT and the UNetT share: the packed weights, an LRU cache of sessions (device buffers per shape), the
+    three C entry points (precompute, one forward, the ODE solve) and `__call__`.  A subclass names its C entry points
+    and its session class, and builds its packed weights."""
+
+    _precompute: str; _forward: str; _ode_sample: str   # names of the backbone's C entry points
+    _session_cls: type
+
+    def __init__(self, *, dim, depth, heads, dim_head, dropout, pe_attn_head, device):
+        if dim_head != 64 or dim != heads * dim_head:
+            raise ValueError("libf5b200 supports dim_head == 64 and dim == heads * 64")
+        if dim not in (256, 512, 1024):
+            # the implicit grouped conv reads 64-channel blocks: its dim/16-channel groups must tile them (64 % (dim/16) == 0)
+            raise ValueError(f"libf5b200 supports dim 256, 512 or 1024, not {dim}: the conv position embedding's dim/16-channel "
+                             "groups must tile 64-channel blocks (see check_common in csrc/dit.cu)")
+        # pe_attn_head: only the first pe_attn_head heads of q and of k are rotated (upstream's name; None = every head)
+        if pe_attn_head is not None and (isinstance(pe_attn_head, bool) or not isinstance(pe_attn_head, int)
+                                         or not 1 <= pe_attn_head <= heads):
+            raise ValueError(f"pe_attn_head must be None (all heads) or an int in 1..{heads}, not {pe_attn_head!r}")
+        if dropout != 0.0:
+            raise NotImplementedError("inference path: dropout must be 0")
+        self.dim, self.depth = dim, depth
+        self.device = torch.device(device)
+        self.packed = None
+        self._sessions: Dict[tuple, object] = {}
+        self.session_cache_size = 12
+
+    # -- weights --
+    def _new_packed(self):
+        """The subclass's packed weights, allocated and not filled."""
+        raise NotImplementedError
+
+    def allocate_weights(self):
+        """Allocate the packed buffer without filling it (non-source ranks before the broadcast)."""
+        self.packed = self._new_packed()
+        return self
+
+    def _require_weights(self):
+        if self.packed is None:
+            raise RuntimeError(f"{type(self).__name__} has no weights: call load_weights() first")
+        return self.packed
+
+    # -- sessions --
+    def _session_args(self) -> tuple:
+        """The session constructor's arguments after `masked`."""
+        return ()
+
+    def _session_key(self) -> tuple:
+        """What a cached session depends on besides its shape."""
+        return self._session_args()
+
+    def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int,
+                masked: bool, bucketed: bool = False):
+        key = (batch, frames, n_times, use_cfg, text_cols, masked, bucketed) + self._session_key()
+        s = self._sessions.pop(key, None)
+        if s is None:
+            while len(self._sessions) >= self.session_cache_size:
+                self._sessions.pop(next(iter(self._sessions)))
+            s = self._session_cls(self.config, self._require_weights().ct_ld, batch, frames, n_times, use_cfg,
+                                  text_cols, self.device, masked, *self._session_args())
+            if bucketed:
+                s.use_bucketing()
+        self._sessions[key] = s          # LRU order: most recently used last
+        return s
+
+    def release_session(self, s) -> None:
+        for k, v in list(self._sessions.items()):
+            if v is s:
+                del self._sessions[k]
+
+    # -- the C entry points --
+    def precompute(self, s) -> None:
+        _lib.check(getattr(_lib.load(), self._precompute)(C.byref(self._require_weights().c_struct()), C.byref(s.c),
+                                                          _stream()))
+
+    def forward_session(self, s, time_index: int) -> torch.Tensor:
+        """One evaluation; returns the session's v (the UNetT's includes each utterance's time row)."""
+        _lib.check(getattr(_lib.load(), self._forward)(C.byref(self._require_weights().c_struct()), C.byref(s.c),
+                                                       int(time_index), _stream()))
+        return s.v
+
+    def ode_sample(self, s, t_grid: torch.Tensor, steps: int, method: int, cfg_strength: float,
+                   y: torch.Tensor, trajectory: Optional[torch.Tensor], scratch: Optional[torch.Tensor]) -> None:
+        """The fixed-grid solve on this backbone (t_grid: host fp32)."""
+        tg = t_grid.numpy().ctypes.data_as(C.POINTER(C.c_float))
+        _lib.check(getattr(_lib.load(), self._ode_sample)(
+            C.byref(self._require_weights().c_struct()), C.byref(s.c), tg, steps, method, C.c_float(cfg_strength),
+            C.c_void_p(y.data_ptr()), C.c_void_p(trajectory.data_ptr()) if trajectory is not None else None,
+            C.c_void_p(scratch.data_ptr()) if scratch is not None else None, _stream()))
+
+    def __call__(self, x: torch.Tensor, cond: torch.Tensor, text: torch.Tensor, time: torch.Tensor,
+                 drop_audio_cond: bool = False, drop_text: bool = False,
+                 mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """One flow-field evaluation, dit.py:374-401.  x, cond: (b, n, mel) fp32; text: (b, nt) int,
+        pad -1; time: scalar or (b,) with equal entries; mask: (b, n) bool prefix mask or None.  Returns (b, n, mel)."""
+        if not x.is_cuda:
+            raise _lib.F5Error(f"{type(self).__name__} needs CUDA tensors: there is no CPU path")
+        b, n, d = x.shape
+        time = torch.as_tensor(time, dtype=torch.float32).reshape(-1)
+        if time.numel() > 1 and not torch.all(time == time[0]):
+            raise NotImplementedError("per-utterance time values are not on the inference path")
+        text = text.to(self.device)
+        _check_prefix_padding(text)
+        s = self.session(b, n, 1, False, text.shape[1], mask is not None)
+        seq_len = None
+        if mask is not None:
+            seq_len = mask.sum(dim=-1)
+            expect = torch.arange(n, device=mask.device)[None, :] < seq_len[:, None]
+            if not torch.equal(mask.bool(), expect):
+                raise ValueError("mask must be a prefix (lens_to_mask) mask")
+        s.set_inputs(text, cond.float(), time[:1].to(self.device), seq_len)
+        s.c.drop_flags = (1 if drop_audio_cond else 0) | (2 if drop_text else 0)
+        s.y_bf16.zero_()
+        s.y_bf16[:, :d].copy_(x.reshape(b * n, d))
+        self.precompute(s)
+        v = self.forward_session(s, 0)
+        return v.view(b, -1, d)[:, -n:].clone()   # the UNetT's v has a time row in front of each utterance
+
+
+class DiT(Backbone):
     """Drop-in for f5_tts_mlx.dit.DiT (inference only)."""
+
+    _precompute, _forward, _ode_sample = "f5_dit_precompute", "f5_dit_forward", "f5_ode_sample"
+    _session_cls = DitSession
 
     def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.0, ff_mult=4, mel_dim=100,
                  text_num_embeds=256, text_dim=None, text_mask_padding=True, conv_layers=0,
@@ -160,24 +286,14 @@ class DiT:
                  fp8_scaling: str = "tensor", fp8_attention: bool = False):
         if text_dim is None:
             text_dim = mel_dim
-        if dim_head != 64 or dim != heads * dim_head:
-            raise ValueError("libf5b200 supports dim_head == 64 and dim == heads * 64")
-        if dim not in (256, 512, 1024):
-            # the implicit grouped conv reads 64-channel blocks: its dim/16-channel groups must tile them (64 % (dim/16) == 0)
-            raise ValueError(f"libf5b200 supports dim 256, 512 or 1024, not {dim}: the conv position embedding's dim/16-channel "
-                             "groups must tile 64-channel blocks (see check_common in csrc/dit.cu)")
+        super().__init__(dim=dim, depth=depth, heads=heads, dim_head=dim_head, dropout=dropout,
+                         pe_attn_head=pe_attn_head, device=device)
         # text_mask_padding=False and pe_attn_head=1 are the F5TTS_Base (v0) model: filler text tokens are not masked,
-        # and only the first head of q and of k is rotated (upstream's pe_attn_head; None = every head)
-        if pe_attn_head is not None and (isinstance(pe_attn_head, bool) or not isinstance(pe_attn_head, int)
-                                         or not 1 <= pe_attn_head <= heads):
-            raise ValueError(f"pe_attn_head must be None (all heads) or an int in 1..{heads}, not {pe_attn_head!r}")
-        if dropout != 0.0:
-            raise NotImplementedError("inference path: dropout must be 0")
+        # and only the first head of q and of k is rotated
         self.config = DiTConfig(dim=dim, depth=depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult,
                                 mel_dim=mel_dim, text_num_embeds=text_num_embeds, text_dim=text_dim,
                                 conv_layers=conv_layers, text_mask_padding=bool(text_mask_padding),
                                 pe_attn_head=pe_attn_head)
-        self.dim, self.depth = dim, depth
         # AdaLN LayerNorm+modulate folded into the neighbouring GEMM epilogues (default); False keeps the separate
         # f5_ln_modulate launches (kept for A/B measurements and as a cross-check in the tests)
         self.fused_adaln = bool(fused_adaln)
@@ -200,97 +316,21 @@ class DiT:
         if fp8_attention and not self.fp8_block:
             raise ValueError('fp8_attention=True needs fp8=True and fp8_scaling="block" (its scales are per (row, head))')
         self.fp8_attention = bool(fp8_attention)
-        self.device = torch.device(device)
-        self.packed: Optional[PackedDiT] = None
-        self._sessions: Dict[tuple, DitSession] = {}
-        self.session_cache_size = 12
 
-    # -- weights --
     def load_weights(self, weights: Weights | list) -> "DiT":
         """Accepts the MLX-named parameter dict (or list of pairs, like mlx `load_weights`); names may
         carry or omit the leading 'transformer.' (the reference loads them through F5TTS)."""
         W = dict(weights)
         if not any(k.startswith("transformer.") for k in W):
             W = {"transformer." + k: v for k, v in W.items()}
-        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8, fp8_scaling=self.fp8_scaling).load(W)
+        self.packed = self._new_packed().load(W)
         return self
 
-    def allocate_weights(self) -> "DiT":
-        """Allocate the packed buffer without filling it (non-source ranks before the broadcast)."""
-        self.packed = PackedDiT(self.config, self.device, fp8=self.fp8, fp8_scaling=self.fp8_scaling)
-        return self
+    def _new_packed(self) -> PackedDiT:
+        return PackedDiT(self.config, self.device, fp8=self.fp8, fp8_scaling=self.fp8_scaling)
 
-    def _require_weights(self) -> PackedDiT:
-        if self.packed is None:
-            raise RuntimeError("DiT has no weights: call load_weights() first")
-        return self.packed
+    def _session_args(self) -> tuple:
+        return (self.fused_adaln, self.fp8, self.fp8_block, self.fp8_attention)
 
-    # -- sessions --
-    def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int,
-                masked: bool, bucketed: bool = False) -> DitSession:
-        key = (batch, frames, n_times, use_cfg, text_cols, masked, self.fused_adaln, bucketed, self.fp8, self.fp8_block,
-               self.fp8_attention, self.config.text_mask_padding, self.config.pe_attn_head)
-        s = self._sessions.pop(key, None)
-        if s is None:
-            while len(self._sessions) >= self.session_cache_size:
-                self._sessions.pop(next(iter(self._sessions)))
-            s = DitSession(self.config, self._require_weights().ct_ld, batch, frames, n_times, use_cfg,
-                           text_cols, self.device, masked, self.fused_adaln, self.fp8, self.fp8_block, self.fp8_attention)
-            if bucketed:
-                s.use_bucketing()
-        self._sessions[key] = s          # LRU order: most recently used last
-        return s
-
-    def release_session(self, s: DitSession) -> None:
-        for k, v in list(self._sessions.items()):
-            if v is s:
-                del self._sessions[k]
-
-    def precompute(self, s: DitSession) -> None:
-        lib = _lib.load()
-        _lib.check(lib.f5_dit_precompute(C.byref(self._require_weights().c_struct()), C.byref(s.c),
-                                         C.c_void_p(torch.cuda.current_stream().cuda_stream)))
-
-    def forward_session(self, s: DitSession, time_index: int) -> torch.Tensor:
-        lib = _lib.load()
-        _lib.check(lib.f5_dit_forward(C.byref(self._require_weights().c_struct()), C.byref(s.c),
-                                      int(time_index), C.c_void_p(torch.cuda.current_stream().cuda_stream)))
-        return s.v
-
-    def ode_sample(self, s: DitSession, t_grid: torch.Tensor, steps: int, method: int, cfg_strength: float,
-                   y: torch.Tensor, trajectory: Optional[torch.Tensor], scratch: Optional[torch.Tensor]) -> None:
-        """f5_ode_sample: the fixed-grid solve on this backbone (t_grid: host fp32)."""
-        tg = t_grid.numpy().ctypes.data_as(C.POINTER(C.c_float))
-        _lib.check(_lib.load().f5_ode_sample(
-            C.byref(self._require_weights().c_struct()), C.byref(s.c), tg, steps, method, C.c_float(cfg_strength),
-            C.c_void_p(y.data_ptr()), C.c_void_p(trajectory.data_ptr()) if trajectory is not None else None,
-            C.c_void_p(scratch.data_ptr()) if scratch is not None else None,
-            C.c_void_p(torch.cuda.current_stream().cuda_stream)))
-
-    def __call__(self, x: torch.Tensor, cond: torch.Tensor, text: torch.Tensor, time: torch.Tensor,
-                 drop_audio_cond: bool = False, drop_text: bool = False,
-                 mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """One flow-field evaluation, dit.py:374-401.  x, cond: (b, n, mel) fp32; text: (b, nt) int,
-        pad -1; time: scalar or (b,) with equal entries; mask: (b, n) bool or None."""
-        if not x.is_cuda:
-            raise _lib.F5Error("DiT needs CUDA tensors: there is no CPU path")
-        b, n, d = x.shape
-        time = torch.as_tensor(time, dtype=torch.float32).reshape(-1)
-        if time.numel() > 1 and not torch.all(time == time[0]):
-            raise NotImplementedError("per-utterance time values are not on the inference path")
-        text = text.to(self.device)
-        _check_prefix_padding(text)
-        s = self.session(b, n, 1, False, text.shape[1], mask is not None)
-        seq_len = None
-        if mask is not None:
-            seq_len = mask.sum(dim=-1)
-            expect = torch.arange(n, device=mask.device)[None, :] < seq_len[:, None]
-            if not torch.equal(mask.bool(), expect):
-                raise ValueError("mask must be a prefix (lens_to_mask) mask")
-        s.set_inputs(text, cond.float(), time[:1].to(self.device), seq_len)
-        s.c.drop_flags = (1 if drop_audio_cond else 0) | (2 if drop_text else 0)
-        s.y_bf16.zero_()
-        s.y_bf16[:, :d].copy_(x.reshape(b * n, d))
-        self.precompute(s)
-        v = self.forward_session(s, 0)
-        return v.view(b, n, d).clone()
+    def _session_key(self) -> tuple:
+        return self._session_args() + (self.config.text_mask_padding, self.config.pe_attn_head)

@@ -1,7 +1,7 @@
 """UNetT — the flat UNet-Transformer backbone of upstream F5-TTS's E2TTS_Base (f5_tts/model/backbones/unett.py).
 
-Same constructor arguments as upstream's UNetT and the `DiT` duck type `F5TTS` uses (`session`, `precompute`,
-`forward_session`, `ode_sample`, `__call__`, `device`, `dim`); all arithmetic runs in libf5b200 (f5_unett_*, sm_90a).
+Same constructor arguments as upstream's UNetT; the sessions, C entry points and `__call__` that `F5TTS` uses come from
+`dit.Backbone`, shared with the DiT.  All arithmetic runs in libf5b200 (f5_unett_*, sm_90a).
 Only the E2TTS_Base form is built: skip_connect_type "concat", no qk_norm, conv_layers 0 (no ConvNeXt, no position
 table), text_mask_padding False, an even depth.  Forward of x, cond [b, n, mel]:
 
@@ -22,14 +22,13 @@ from __future__ import annotations
 import ctypes as C
 import math
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Optional
 
 import numpy as np
 import torch
 
-from . import _lib
-from .dit import _check_prefix_padding, rope_table
-from .weights import (DitBlockWeightsC, Weights, _normal, _round_up, _Spec, _uniform, pack_grouped_conv)
+from .dit import Backbone, rope_table
+from .weights import DitBlockWeightsC, PackedWeights, Weights, _normal, _uniform, pack_grouped_conv
 
 
 @dataclass(frozen=True)
@@ -152,25 +151,8 @@ class UNetTBuffersC(C.Structure):
                                           "c_bf16", "qkv_bf16", "ff_bf16", "ln_stats", "skip", "v")]
 
 
-class PackedUNetT:
-    """Packed UNetT weights in one device buffer (so that the multi-GPU path is one broadcast) + the ctypes view."""
-
-    ALIGN = 256
-
-    def __init__(self, cfg: UNetTConfig, device: torch.device | str = "cuda"):
-        self.cfg = cfg
-        self.device = torch.device(device)
-        self.ct_ld = _round_up(cfg.mel_dim + cfg.text_dim, 64)
-        self.specs: Dict[str, _Spec] = {}
-        off = 0
-        for name, shape, dtype in self._layout():
-            nbytes = int(np.prod(shape)) * (2 if dtype == torch.bfloat16 else 4)
-            self.specs[name] = _Spec(name, tuple(shape), dtype, off)
-            off = _round_up(off + nbytes, self.ALIGN)
-        self.nbytes = off
-        self.buffer = torch.zeros(self.nbytes, dtype=torch.uint8, device=self.device)
-        self._c: Optional[UNetTWeightsC] = None
-        self._keep: list = []
+class PackedUNetT(PackedWeights):
+    """Packed UNetT weights in one device buffer + the ctypes view libf5b200 takes."""
 
     def _layout(self):
         c = self.cfg
@@ -199,16 +181,6 @@ class PackedUNetT:
         yield "skip_w", (c.depth // 2, D, 2 * D), bf
         yield "proj_w", (c.mel_dim, D), bf
         yield "proj_b", (c.mel_dim,), f32
-
-    def view(self, name: str) -> torch.Tensor:
-        s = self.specs[name]
-        nbytes = int(np.prod(s.shape)) * (2 if s.dtype == torch.bfloat16 else 4)
-        return self.buffer[s.offset:s.offset + nbytes].view(s.dtype).view(s.shape)
-
-    def _put(self, name: str, t: torch.Tensor) -> None:
-        v = self.view(name)
-        assert tuple(t.shape) == tuple(v.shape), (name, t.shape, v.shape)
-        v.copy_(t.to(v.dtype))
 
     def load(self, W: Weights) -> "PackedUNetT":
         """Fill the buffer from checkpoint_state() weights (fp32), folding each RMSNorm gain into its consumer."""
@@ -248,12 +220,6 @@ class PackedUNetT:
         self._put("skip_w", skip)
         self._put("proj_w", g(T + "proj_out.weight") * g(T + "norm_out.g")[None, :])
         self._put("proj_b", g(T + "proj_out.bias"))
-        return self
-
-    def broadcast(self, src: int = 0) -> "PackedUNetT":
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            dist.broadcast(self.buffer, src=src)
         return self
 
     def c_struct(self) -> UNetTWeightsC:
@@ -353,12 +319,11 @@ class UNetTSession:
             self.seq_len1.copy_(self.seq_len + 1)
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-class UNetT:
+class UNetT(Backbone):
     """Drop-in for upstream F5-TTS's UNetT (inference only) in its E2TTS_Base form."""
+
+    _precompute, _forward, _ode_sample = "f5_unett_precompute", "f5_unett_forward", "f5_unett_ode_sample"
+    _session_cls = UNetTSession
 
     def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.0, ff_mult=4, mel_dim=100,
                  text_num_embeds=256, text_dim=None, text_mask_padding=False, qk_norm=None, conv_layers=0,
@@ -375,101 +340,18 @@ class UNetT:
             raise ValueError("text_mask_padding=True is not built: E2TTS_Base keeps filler tokens unmasked")
         if not isinstance(depth, int) or depth <= 0 or depth % 2:
             raise ValueError(f"depth must be a positive even number (the skips pair layer i with depth - 1 - i), not {depth!r}")
-        if dim_head != 64 or dim != heads * dim_head:
-            raise ValueError("libf5b200 supports dim_head == 64 and dim == heads * 64")
-        if dim not in (256, 512, 1024):
-            raise ValueError(f"libf5b200 supports dim 256, 512 or 1024, not {dim}")
         if text_dim % 4:
             raise ValueError(f"text_dim must be a multiple of 4, not {text_dim}")
-        if pe_attn_head is not None and (isinstance(pe_attn_head, bool) or not isinstance(pe_attn_head, int)
-                                         or not 1 <= pe_attn_head <= heads):
-            raise ValueError(f"pe_attn_head must be None (all heads) or an int in 1..{heads}, not {pe_attn_head!r}")
-        if dropout != 0.0:
-            raise NotImplementedError("inference path: dropout must be 0")
+        super().__init__(dim=dim, depth=depth, heads=heads, dim_head=dim_head, dropout=dropout,
+                         pe_attn_head=pe_attn_head, device=device)
         self.config = UNetTConfig(dim=dim, depth=depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult,
                                   mel_dim=mel_dim, text_num_embeds=text_num_embeds, text_dim=text_dim,
                                   pe_attn_head=pe_attn_head)
-        self.dim, self.depth = dim, depth
-        self.device = torch.device(device)
-        self.packed: Optional[PackedUNetT] = None
-        self._sessions: Dict[tuple, UNetTSession] = {}
-        self.session_cache_size = 12
 
     def load_weights(self, weights: Weights) -> "UNetT":
         """Upstream-named weights (an upstream state dict: see checkpoint_state, which this applies)."""
-        self.packed = PackedUNetT(self.config, self.device).load(checkpoint_state(dict(weights), self.config))
+        self.packed = self._new_packed().load(checkpoint_state(dict(weights), self.config))
         return self
 
-    def allocate_weights(self) -> "UNetT":
-        self.packed = PackedUNetT(self.config, self.device)
-        return self
-
-    def _require_weights(self) -> PackedUNetT:
-        if self.packed is None:
-            raise RuntimeError("UNetT has no weights: call load_weights() first")
-        return self.packed
-
-    def session(self, batch: int, frames: int, n_times: int, use_cfg: bool, text_cols: int, masked: bool,
-                bucketed: bool = False) -> UNetTSession:
-        key = (batch, frames, n_times, use_cfg, text_cols, masked, bucketed)
-        s = self._sessions.pop(key, None)
-        if s is None:
-            while len(self._sessions) >= self.session_cache_size:
-                self._sessions.pop(next(iter(self._sessions)))
-            s = UNetTSession(self.config, self._require_weights().ct_ld, batch, frames, n_times, use_cfg, text_cols,
-                             self.device, masked)
-            if bucketed:
-                s.use_bucketing()
-        self._sessions[key] = s
-        return s
-
-    def release_session(self, s: UNetTSession) -> None:
-        for k, v in list(self._sessions.items()):
-            if v is s:
-                del self._sessions[k]
-
-    def precompute(self, s: UNetTSession) -> None:
-        _lib.check(_lib.load().f5_unett_precompute(C.byref(self._require_weights().c_struct()), C.byref(s.c), _stream()))
-
-    def forward_session(self, s: UNetTSession, time_index: int) -> torch.Tensor:
-        """One evaluation; returns the session's v [rows1, mel] (the time rows included)."""
-        _lib.check(_lib.load().f5_unett_forward(C.byref(self._require_weights().c_struct()), C.byref(s.c),
-                                                int(time_index), _stream()))
-        return s.v
-
-    def ode_sample(self, s: UNetTSession, t_grid: torch.Tensor, steps: int, method: int, cfg_strength: float,
-                   y: torch.Tensor, trajectory: Optional[torch.Tensor], scratch: Optional[torch.Tensor]) -> None:
-        """f5_unett_ode_sample: the fixed-grid solve on this backbone (t_grid: host fp32)."""
-        tg = t_grid.numpy().ctypes.data_as(C.POINTER(C.c_float))
-        _lib.check(_lib.load().f5_unett_ode_sample(
-            C.byref(self._require_weights().c_struct()), C.byref(s.c), tg, steps, method, C.c_float(cfg_strength),
-            C.c_void_p(y.data_ptr()), C.c_void_p(trajectory.data_ptr()) if trajectory is not None else None,
-            C.c_void_p(scratch.data_ptr()) if scratch is not None else None, _stream()))
-
-    def __call__(self, x: torch.Tensor, cond: torch.Tensor, text: torch.Tensor, time: torch.Tensor,
-                 drop_audio_cond: bool = False, drop_text: bool = False,
-                 mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """One flow-field evaluation.  x, cond: (b, n, mel) fp32; text: (b, nt) int, pad -1; time: scalar or (b,) with
-        equal entries; mask: (b, n) bool prefix mask or None.  Returns (b, n, mel)."""
-        if not x.is_cuda:
-            raise _lib.F5Error("UNetT needs CUDA tensors: there is no CPU path")
-        b, n, d = x.shape
-        time = torch.as_tensor(time, dtype=torch.float32).reshape(-1)
-        if time.numel() > 1 and not torch.all(time == time[0]):
-            raise NotImplementedError("per-utterance time values are not on the inference path")
-        text = text.to(self.device)
-        _check_prefix_padding(text)
-        s = self.session(b, n, 1, False, text.shape[1], mask is not None)
-        seq_len = None
-        if mask is not None:
-            seq_len = mask.sum(dim=-1)
-            expect = torch.arange(n, device=mask.device)[None, :] < seq_len[:, None]
-            if not torch.equal(mask.bool(), expect):
-                raise ValueError("mask must be a prefix (lens_to_mask) mask")
-        s.set_inputs(text, cond.float(), time[:1].to(self.device), seq_len)
-        s.c.drop_flags = (1 if drop_audio_cond else 0) | (2 if drop_text else 0)
-        s.y_bf16.zero_()
-        s.y_bf16[:, :d].copy_(x.reshape(b * n, d))
-        self.precompute(s)
-        v = self.forward_session(s, 0)
-        return v.view(b, n + 1, d)[:, 1:].clone()
+    def _new_packed(self) -> PackedUNetT:
+        return PackedUNetT(self.config, self.device)

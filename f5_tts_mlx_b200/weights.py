@@ -384,21 +384,16 @@ class _Spec:
     offset: int = 0
 
 
-class PackedDiT:
-    """Packed DiT weights living in one device buffer + the ctypes view libf5b200 takes."""
+class PackedWeights:
+    """A backbone's packed weights in one device buffer, so that the multi-GPU path is one broadcast.  Each tensor sits
+    at an ALIGN-byte aligned offset in the order the subclass's `_layout()` yields (name, shape, dtype) triples; the
+    layout depends on the config only, so every rank derives the same one.  Subclasses add `load` and `c_struct`."""
 
     ALIGN = 256
 
-    def __init__(self, cfg: DiTConfig, device: torch.device | str = "cuda", fp8: bool = False,
-                 fp8_scaling: str = "tensor"):
+    def __init__(self, cfg, device: torch.device | str = "cuda"):
         self.cfg = cfg
         self.device = torch.device(device)
-        self.fp8 = bool(fp8)           # also keep e4m3 copies of the QKV / FF1 weights (appended after the bf16 layout)
-        if fp8_scaling not in FP8_SCALINGS:
-            raise ValueError(f"fp8_scaling must be one of {FP8_SCALINGS}, not {fp8_scaling!r}")
-        # "tensor": one scale per weight tensor; "block": one power-of-two scale per output channel (the block-scaled mode)
-        self.fp8_scaling = fp8_scaling
-        self.fp8_block = self.fp8 and fp8_scaling == "block"
         self.ct_ld = _round_up(cfg.mel_dim + cfg.text_dim, 64)
         self.specs: Dict[str, _Spec] = {}
         off = 0
@@ -408,10 +403,46 @@ class PackedDiT:
             off = _round_up(off + nbytes, self.ALIGN)
         self.nbytes = off
         self.buffer = torch.zeros(self.nbytes, dtype=torch.uint8, device=self.device)
-        self._c: Optional[DitWeightsC] = None
+        self._c = None
         self._keep: list = []
 
-    # -- layout: depends on the config only, so every rank derives the same one --
+    @staticmethod
+    def _esize(dtype) -> int:
+        return {torch.bfloat16: 2, torch.uint8: 1}.get(dtype, 4)
+
+    def view(self, name: str) -> torch.Tensor:
+        s = self.specs[name]
+        n = int(np.prod(s.shape))
+        nbytes = n * self._esize(s.dtype)
+        return self.buffer[s.offset:s.offset + nbytes].view(s.dtype).view(s.shape)
+
+    def _put(self, name: str, t: torch.Tensor) -> None:
+        v = self.view(name)
+        assert tuple(t.shape) == tuple(v.shape), (name, t.shape, v.shape)
+        v.copy_(t.to(v.dtype))
+
+    def broadcast(self, src: int = 0):
+        """The ONE collective of the multi-GPU path: rank `src` holds the packed weights, every
+        other rank receives them (NCCL over NVLink when the process group is nccl)."""
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            dist.broadcast(self.buffer, src=src)
+        return self
+
+
+class PackedDiT(PackedWeights):
+    """Packed DiT weights living in one device buffer + the ctypes view libf5b200 takes."""
+
+    def __init__(self, cfg: DiTConfig, device: torch.device | str = "cuda", fp8: bool = False,
+                 fp8_scaling: str = "tensor"):
+        self.fp8 = bool(fp8)           # also keep e4m3 copies of the QKV / FF1 weights (appended after the bf16 layout)
+        if fp8_scaling not in FP8_SCALINGS:
+            raise ValueError(f"fp8_scaling must be one of {FP8_SCALINGS}, not {fp8_scaling!r}")
+        # "tensor": one scale per weight tensor; "block": one power-of-two scale per output channel (the block-scaled mode)
+        self.fp8_scaling = fp8_scaling
+        self.fp8_block = self.fp8 and fp8_scaling == "block"
+        super().__init__(cfg, device)
+
     def _layout(self):
         c = self.cfg
         D, F, Ct, Ci = c.dim, c.ff_inner, c.text_dim, 2 * c.text_dim
@@ -464,21 +495,6 @@ class PackedDiT:
                 yield f"blk{i}.out_w8", (D, D), torch.uint8
                 yield f"blk{i}.ff2_w8", (D, F), torch.uint8
             yield "fp8_scales", (c.depth, 4), f32       # (qkv, ff1, out, ff2) per block: travels with the ONE broadcast
-
-    @staticmethod
-    def _esize(dtype) -> int:
-        return {torch.bfloat16: 2, torch.uint8: 1}.get(dtype, 4)
-
-    def view(self, name: str) -> torch.Tensor:
-        s = self.specs[name]
-        n = int(np.prod(s.shape))
-        nbytes = n * self._esize(s.dtype)
-        return self.buffer[s.offset:s.offset + nbytes].view(s.dtype).view(s.shape)
-
-    def _put(self, name: str, t: torch.Tensor) -> None:
-        v = self.view(name)
-        assert tuple(t.shape) == tuple(v.shape), (name, t.shape, v.shape)
-        v.copy_(t.to(v.dtype))
 
     def load(self, W: Weights) -> "PackedDiT":
         """Fill the buffer from an MLX-named parameter dict (fp32)."""
@@ -546,14 +562,6 @@ class PackedDiT:
                     self.view("fp8_scales")[i, j] = sc
         self._put("proj_w", g(T + "proj_out.weight"))
         self._put("proj_b", g(T + "proj_out.bias"))
-        return self
-
-    def broadcast(self, src: int = 0) -> "PackedDiT":
-        """The ONE collective of the multi-GPU path: rank `src` holds the packed weights, every
-        other rank receives them (NCCL over NVLink when the process group is nccl)."""
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            dist.broadcast(self.buffer, src=src)
         return self
 
     def c_struct(self) -> DitWeightsC:

@@ -1,6 +1,7 @@
-"""Launch trace of the DiT, ODE sampler and duration predictor host code, made on the CPU; launch_trace_digests.txt.
+"""Launch trace of the DiT, UNetT, ODE sampler and duration predictor host code, made on the CPU;
+launch_trace_digests.txt.
 
-csrc/dit.cu and csrc/duration.cu hold no kernels.  Compiled with the library's nvcc flags and linked against
+csrc/dit.cu, csrc/unett.cu and csrc/duration.cu hold no kernels.  Compiled with the library's nvcc flags and linked against
 tests/host_trace/stubs.cu instead of the rest of the library, they run without a GPU, and every launch they make is
 printed with all of its arguments (see stubs.cu for the cases).  The full trace is about 2 MB of text, so the fixture
 keeps one line per case: the first 16 hex digits of the SHA-256 of the case's trace (its header, every launch line
@@ -27,6 +28,7 @@ if ROOT not in sys.path:
 FIXTURE = os.path.join(HERE, "launch_trace_digests.txt")
 SOURCES = [os.path.join(ROOT, "f5_tts_mlx_b200", "csrc", "dit.cu"),
            os.path.join(ROOT, "f5_tts_mlx_b200", "csrc", "duration.cu"),
+           os.path.join(ROOT, "f5_tts_mlx_b200", "csrc", "unett.cu"),
            os.path.join(ROOT, "tests", "host_trace", "stubs.cu")]
 
 

@@ -1,11 +1,12 @@
-// Launch trace of the DiT, ODE sampler and duration predictor host code, without a GPU.
+// Launch trace of the DiT, UNetT, ODE sampler and duration predictor host code, without a GPU.
 //
-// csrc/dit.cu and csrc/duration.cu contain no kernels: they only decide which launchers run, in which order, with
-// which arguments.  Linked against this file instead of the rest of the library, every launcher they call prints
-// itself with all of its arguments, and main() runs f5_dit_precompute / f5_dit_forward / f5_ode_sample /
-// f5_duration_forward over every mode and binding the forwards distinguish.  The output is the launch sequence those
-// entry points issue, so two versions of the host code launch the same work exactly when their traces are equal
-// (tests/test_host_launch_trace.py, tests/golden/make_launch_trace.py).
+// csrc/dit.cu, csrc/unett.cu and csrc/duration.cu contain no kernels: they only decide which launchers run, in which
+// order, with which arguments.  Linked against this file instead of the rest of the library, every launcher they call
+// prints itself with all of its arguments, and main() runs f5_dit_precompute / f5_dit_forward / f5_ode_sample /
+// f5_duration_forward / f5_unett_precompute / f5_unett_forward / f5_unett_ode_sample over every mode and binding the
+// forwards distinguish.  The output is the launch sequence those entry points issue, so two versions of the host code
+// launch the same work exactly when their traces are equal (tests/test_host_launch_trace.py,
+// tests/golden/make_launch_trace.py).
 //
 // Nothing is dereferenced on the device side, so each pointer field gets a slot of its own in an address range that
 // is never touched; a pointer prints as its slot's name plus the byte offset into it (`b.ln_tab+0x1a0`), never as an
@@ -71,7 +72,7 @@ struct Line {
 
 }  // namespace
 
-// ---------------- recording stubs of everything dit.o and duration.o link against ----------------
+// ---------------- recording stubs of everything dit.o, unett.o and duration.o link against ----------------
 namespace f5 {
 
 int set_error(int code, const char* fmt, ...) {
@@ -120,11 +121,13 @@ int launch_time_mlp(const float* tvals, int T, int D, const float* w0, const flo
 }
 
 int launch_ode_update(const OdeUpdateParams& u, cudaStream_t st) {
-  return Line("launch_ode_update").p("v", u.v).i("ldv", u.ldv).i("null_row_offset", u.null_row_offset)
+  Line l("launch_ode_update");
+  l.p("v", u.v).i("ldv", u.ldv).i("null_row_offset", u.null_row_offset)
       .f("cfg_strength", u.cfg_strength).p("y_base", u.y_base).p("y_out", u.y_out).f("a", u.a).p("k_acc", u.k_acc)
       .f("acc_w", u.acc_w).i("acc_init", u.acc_init).i("use_acc", u.use_acc).p("y_bf16", u.y_bf16)
-      .i("ld_bf16", u.ld_bf16).i("bf16_copy_row_offset", u.bf16_copy_row_offset).i("rows", u.rows).i("d", u.d)
-      .p("st", st).done();
+      .i("ld_bf16", u.ld_bf16).i("bf16_copy_row_offset", u.bf16_copy_row_offset).i("rows", u.rows).i("d", u.d);
+  if (u.v_frames) l.i("v_frames", u.v_frames);   // UNetT only: 0 (left out) for the DiT
+  return l.p("st", st).done();
 }
 
 int launch_cast_pad_bf16(const float* src, int d, void* dst, int ld, int rows, long long copy_row_offset,
@@ -151,6 +154,12 @@ int launch_duration_head(const float* x, int B, int N, int D, const int* len, co
       .p("pred_w", pred_w).p("out", out).p("st", st).done();
 }
 
+int launch_unett_time_pack(const float* xe, const float* t_emb, float* x, void* x_bf16, long long ld_bf16,
+                           float* ln_stats, int BU, int N, int D, cudaStream_t st) {
+  return Line("launch_unett_time_pack").p("xe", xe).p("t_emb", t_emb).p("x", x).p("x_bf16", x_bf16)
+      .i("ld_bf16", ld_bf16).p("ln_stats", ln_stats).i("BU", BU).i("N", N).i("D", D).p("st", st).done();
+}
+
 }  // namespace f5
 
 // Every field of f5_gemm_args in declaration order.  A field that is zero (all bits) is left out: the host code
@@ -168,12 +177,12 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* g, void* st) {
   p("resid", g->resid); i("ldr", g->ldr); p("gate", g->gate); p("row_len", g->row_len);
   p("rope", g->rope); i("rope_cols", g->rope_cols); f("q_scale", g->q_scale); i("q_cols", g->q_cols);
   i("tile_n", g->tile_n); p("out2_bf16", g->out2_bf16); i("ldo2", g->ldo2); i("w_static", g->w_static);
-  p("prefetch", g->prefetch); i("prefetch_bytes", g->prefetch_bytes);
+  i("ln_rms", g->ln_rms); p("prefetch", g->prefetch); i("prefetch_bytes", g->prefetch_bytes);
   p("ln_scale", g->ln_scale); p("ln_stats", g->ln_stats); p("ln_in_stats", g->ln_in_stats); p("ln_tab", g->ln_tab);
   i("ln_tab_ld", g->ln_tab_ld);
   i("ab_fp8", g->ab_fp8); i("out2_fp8", g->out2_fp8); f("acc_scale", g->acc_scale); i("out_fp8", g->out_fp8);
   p("a_scale", g->a_scale); i("a_scale_ld", g->a_scale_ld); p("w_scale", g->w_scale); p("out_scale", g->out_scale);
-  p("out2_scale", g->out2_scale);
+  p("out2_scale", g->out2_scale); i("rope_col2", g->rope_col2); i("conv_dilation", g->conv_dilation);
   return l.p("st", st).done();
 }
 
@@ -411,6 +420,108 @@ void duration_case() {
   printf("f5_duration_forward -> %d\n", f5_duration_forward(&w, &b, kStream));
 }
 
+// depth 4: both skip halves, and the skip-weight prefetch from the first half into the second
+constexpr int kUDepth = 4;
+
+struct UNetT {
+  f5_dit_block_weights blocks[kUDepth];
+  f5_unett_weights w;
+  f5_unett_buffers all;   // every buffer bound
+};
+
+UNetT* make_unett() {
+  UNetT* u = new UNetT();
+  for (int l = 0; l < kUDepth; ++l) {
+    f5_dit_block_weights& k = u->blocks[l];
+    k = block("uw.blocks[" + std::to_string(l) + "].", l);
+    k.qkv_w8 = k.ff1_w8 = k.out_w8 = k.ff2_w8 = nullptr;
+    k.qkv_ws = k.ff1_ws = k.out_ws = k.ff2_ws = nullptr;
+    k.qkv_s8 = k.ff1_s8 = k.out_s8 = k.ff2_s8 = 0.f;
+  }
+  f5_unett_weights& w = u->w;
+  memset(&w, 0, sizeof(w));
+  w.dim = kDim; w.depth = kUDepth; w.heads = kHeads; w.ff_inner = kFF; w.mel_dim = kMel; w.text_dim = kText;
+  w.text_rows = 41; w.ct_ld = 256; w.rope_heads = 1;
+#define F(x) w.x = slot("uw." #x)
+  F(time_w0); F(time_b0); F(time_w2); F(time_b2); F(text_emb); F(in_x_w); F(in_ct_w); F(in_b); F(conv_w[0]);
+  F(conv_w[1]); F(conv_b[0]); F(conv_b[1]); F(skip_w); F(proj_w); F(proj_b);
+#undef F
+  w.blocks = u->blocks;
+  f5_unett_buffers& b = u->all;
+  memset(&b, 0, sizeof(b));
+#define F(x) b.x = slot("ub." #x)
+  F(text); F(seq_len1); F(valid_len); F(valid_len1); F(cond); F(tvals); F(rope); F(hoist); F(t_emb); F(text_x);
+  F(ct_bf16); F(silu_t); F(y_bf16); F(h); F(x); F(a_bf16); F(c_bf16); F(qkv_bf16); F(ff_bf16); F(ln_stats); F(skip);
+  F(v);
+#undef F
+  return u;
+}
+
+f5_unett_buffers unett_buffers(const UNetT* u, int cfg, int drop_flags, bool seq_len1, bool valid_len, int frames,
+                               int n_times) {
+  f5_unett_buffers b = u->all;
+  b.batch = kBatch; b.frames = frames; b.cfg = cfg; b.n_times = n_times; b.text_len_max = 24;
+  b.drop_flags = drop_flags;
+  if (!seq_len1) b.seq_len1 = nullptr;
+  if (!valid_len) b.valid_len = b.valid_len1 = nullptr;
+  return b;
+}
+
+void unett_cases(UNetT* u) {
+  for (int cd = 0; cd < 5; ++cd) {   // CFG on, or off with each drop_flags value
+    const int cfg = cd == 0, drop = cd == 0 ? 0 : cd - 1;
+    for (int seq = 1; seq >= 0; --seq)
+      for (int valid = 1; valid >= 0; --valid)
+        for (int frames : kFrames) {
+          const f5_unett_buffers b = unett_buffers(u, cfg, drop, seq, valid, frames, 3);
+          printf("== unett cfg=%d drop_flags=%d seq_len1=%s valid_len=%s batch=%d frames=%d\n", cfg, drop,
+                 bound(b.seq_len1), bound(b.valid_len), b.batch, frames);
+          printf("f5_unett_precompute -> %d\n", f5_unett_precompute(&u->w, &b, kStream));
+          printf("f5_unett_forward(time_index=1) -> %d\n", f5_unett_forward(&u->w, &b, 1, kStream));
+        }
+  }
+  const float grid[3] = {0.f, 0.375f, 1.f};
+  for (int method = 0; method < 3; ++method) {
+    const int per = method == 0 ? 1 : (method == 1 ? 2 : 4);
+    for (int cfg = 1; cfg >= 0; --cfg) {
+      const f5_unett_buffers b = unett_buffers(u, cfg, 0, true, false, kFrames[0], 2 * per);
+      const bool traj = method != 1;   // the midpoint run updates y in place
+      printf("== unett ode method=%d cfg=%d trajectory=%s frames=%d\n", method, cfg, traj ? "bound" : "NULL",
+             b.frames);
+      const int rc = f5_unett_ode_sample(&u->w, &b, grid, 3, method, cfg ? 2.f : 0.f, slot("y"),
+                                         traj ? (float*)slot("trajectory") : nullptr, slot("scratch"), kStream);
+      printf("f5_unett_ode_sample -> %d\n", rc);
+    }
+  }
+}
+
+// what check_unett refuses, before anything is launched
+void unett_rejected_cases(UNetT* u) {
+  struct Case {
+    const char* what;
+    void (*edit)(f5_unett_weights&, f5_unett_buffers&, f5_dit_block_weights*);
+  };
+  const Case cases[] = {
+      {"odd depth", [](f5_unett_weights& w, f5_unett_buffers&, f5_dit_block_weights*) { w.depth = 3; }},
+      {"an FP8 weight in blocks[2]", [](f5_unett_weights&, f5_unett_buffers&, f5_dit_block_weights* k) {
+         k[2].ff1_w8 = slot("uw.blocks[2].ff1_w8");
+       }},
+      {"valid_len without valid_len1",
+       [](f5_unett_weights&, f5_unett_buffers& b, f5_dit_block_weights*) { b.valid_len1 = nullptr; }},
+      {"no skip buffer", [](f5_unett_weights&, f5_unett_buffers& b, f5_dit_block_weights*) { b.skip = nullptr; }},
+  };
+  for (const Case& c : cases) {
+    f5_dit_block_weights blocks[kUDepth];
+    memcpy(blocks, u->blocks, sizeof(blocks));
+    f5_unett_weights w = u->w;
+    w.blocks = blocks;
+    f5_unett_buffers b = unett_buffers(u, 1, 0, true, true, kFrames[0], 3);
+    c.edit(w, b, blocks);
+    printf("== unett rejected: %s\n", c.what);
+    printf("f5_unett_forward(time_index=1) -> %d\n", f5_unett_forward(&w, &b, 1, kStream));
+  }
+}
+
 }  // namespace
 
 int main() {
@@ -419,5 +530,8 @@ int main() {
   ode_cases(d);
   rejected_cases(d);
   duration_case();
+  UNetT* u = make_unett();
+  unett_cases(u);
+  unett_rejected_cases(u);
   return 0;
 }

@@ -1,8 +1,9 @@
-"""The DiT, ODE sampler and duration predictor host code launches exactly the work the committed digests record: the
-same launches in the same order with the same arguments, every f5_gemm_args field included, in each of the five DiT
-modes, with and without CFG, each drop_flags value, seq_len and valid_len bound or not, on both sides of the weight
-prefetch cutoff, for the three solvers, and the same refusals of partly bound modes.  Runs on the CPU: the host code
-is linked against recording stubs (tests/host_trace/stubs.cu, tests/golden/make_launch_trace.py)."""
+"""The DiT, UNetT, ODE sampler and duration predictor host code launches exactly the work the committed digests
+record: the same launches in the same order with the same arguments, every f5_gemm_args field included, in each of the
+five DiT modes and the UNetT, with and without CFG, each drop_flags value, seq_len (UNetT: seq_len1) and valid_len
+bound or not, on both sides of the weight prefetch cutoff, for the three solvers, and the same refusals of partly
+bound DiT modes and of malformed UNetT weights and buffers.  Runs on the CPU: the host code is linked against recording
+stubs (tests/host_trace/stubs.cu, tests/golden/make_launch_trace.py)."""
 import importlib.util
 import os
 
