@@ -148,6 +148,10 @@ SYMBOLS: dict[str, tuple] = {
     "f5_bigvgan_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "f5_bigvgan_act_forward": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                          C.c_int32, C.c_void_p, C.c_void_p]),
+    "f5_bigvgan_resblock_mean": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int64, C.c_int32, C.c_void_p,
+                                           C.c_void_p]),
+    "f5_bigvgan_conv_post": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                       C.c_void_p, C.c_void_p]),
     "f5_resample_table": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_float), C.c_int64]),
     "f5_resample": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                               C.c_int64, C.c_void_p]),

@@ -120,6 +120,27 @@ static int launch_bigvgan_act(const float* x, int batch, int rpb, int C, const i
   return 0;
 }
 
+// the resblock mean of n elements over nk streams stride apart (the decode and its test entry)
+static int launch_bigvgan_mean(const float* xk, long long stride, int nk, long long n, bool out_bf16, void* out,
+                               cudaStream_t st) {
+  if (out_bf16)
+    F5_CHECK_CUDA(launch_kernel(bigvgan_mean_kernel<true>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, xk,
+                                stride, nk, n, out));
+  else
+    F5_CHECK_CUDA(launch_kernel(bigvgan_mean_kernel<false>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, xk,
+                                stride, nk, n, out));
+  F5_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+static int launch_bigvgan_conv_post(const float* x, int batch, int T, int C, const float* w, const float* bias,
+                                    int use_tanh, float* out, cudaStream_t st) {
+  F5_CHECK_CUDA(launch_kernel(bigvgan_conv_post_kernel, dim3(cdiv(T, 256), batch), dim3(256), 0, st, x, T, C, w, bias,
+                              use_tanh, out));
+  F5_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
 static bool act_ok(const f5_bigvgan_act& a) { return a.alpha && a.h_up && a.h_down; }
 
 }  // namespace f5
@@ -230,22 +251,35 @@ int f5_bigvgan_decode(const f5_bigvgan_weights* w, const f5_bigvgan_buffers* b, 
     }
     const long long n = (long long)B * T * C;
     ProfScope ps(PROF_OTHER, 0.0, 4.0 * NK * n + (i + 1 < NU ? 2.0 : 4.0) * n);
-    if (i + 1 < NU)
-      F5_CHECK_CUDA(launch_kernel(bigvgan_mean_kernel<true>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st,
-                                  (const float*)b->xk, stride, NK, n, b->a_bf16));
-    else
-      F5_CHECK_CUDA(launch_kernel(bigvgan_mean_kernel<false>, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st,
-                                  (const float*)b->xk, stride, NK, n, (void*)b->t));
-    F5_CHECK_CUDA(cudaGetLastError());
+    const bool last = i + 1 == NU;
+    if (int e = launch_bigvgan_mean(b->xk, stride, NK, n, !last, last ? (void*)b->t : b->a_bf16, st)) return e;
   }
   if (int e = launch_bigvgan_act(b->t, B, T, C, nullptr, w->act_post, false, b->x_up, st)) return e;
   {
     ProfScope ps(PROF_OTHER, 14.0 * B * (double)T * C, 4.0 * B * (double)T * (C + 1));
-    F5_CHECK_CUDA(launch_kernel(bigvgan_conv_post_kernel, dim3(cdiv(T, 256), B), dim3(256), 0, st, (const float*)b->x_up,
-                                T, C, w->conv_post_w, w->conv_post_b, w->use_tanh_at_final, wave));
-    F5_CHECK_CUDA(cudaGetLastError());
+    if (int e = launch_bigvgan_conv_post(b->x_up, B, T, C, w->conv_post_w, w->conv_post_b, w->use_tanh_at_final, wave,
+                                         st))
+      return e;
   }
   return 0;
+}
+
+int f5_bigvgan_resblock_mean(const float* xk, int64_t stride, int32_t nk, int64_t n, int32_t out_bf16, void* out,
+                             void* stream) {
+  if (int e = device_check()) return e;
+  F5_REQUIRE(xk && out, "f5_bigvgan_resblock_mean: null pointer");
+  F5_REQUIRE(nk >= 1 && n > 0 && (nk == 1 || stride >= n) && (n + 255) / 256 <= INT32_MAX,
+             "f5_bigvgan_resblock_mean: bad shape nk=%d n=%lld stride=%lld", nk, (long long)n, (long long)stride);
+  return launch_bigvgan_mean(xk, stride, nk, n, out_bf16 != 0, out, (cudaStream_t)stream);
+}
+
+int f5_bigvgan_conv_post(const float* x, int32_t batch, int32_t frames, int32_t channels, const float* w,
+                         const float* bias, int32_t use_tanh, float* out, void* stream) {
+  if (int e = device_check()) return e;
+  F5_REQUIRE(x && w && out, "f5_bigvgan_conv_post: null pointer");
+  F5_REQUIRE(batch > 0 && frames > 0 && channels > 0 && batch <= 65535,
+             "f5_bigvgan_conv_post: bad shape batch=%d frames=%d channels=%d", batch, frames, channels);
+  return launch_bigvgan_conv_post(x, batch, frames, channels, w, bias, use_tanh, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

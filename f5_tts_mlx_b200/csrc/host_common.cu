@@ -193,6 +193,6 @@ int f5_struct_sizes(int32_t* out, int32_t n) {
   return 10;
 }
 const char* f5_last_error(void) { return f5::g_err; }
-int f5_abi_version(void) { return 2006; }
+int f5_abi_version(void) { return 2007; }
 int f5_device_check(void) { return f5::device_check(); }
 }

@@ -53,10 +53,12 @@ def gemm(
     conv_taps: int = 1,
     conv_pad: int = 0,
     conv_grouped: bool = False,
+    conv_dilation: int = 0,                # frames between taps (0 or 1: adjacent frames)
     tile_n: int = 0,                       # 0 (auto), 64 or 128
     out2: torch.Tensor | None = None,          # bf16 [rows, >=n] second copy (or the fused-LN operand, see ln_scale)
     ln_scale: torch.Tensor | None = None,      # f32 [n]: producer mode — out2 = bf16(out * (1 + ln_scale)), ln_stats filled
-    ln_stats: torch.Tensor | None = None,      # f32 [rows, n/64, 2] (sum, sum of squares) per 64 columns
+    ln_stats: torch.Tensor | None = None,      # f32 [rows, n/64, 2] (sum, sum of squares) per 64 columns (with or
+                                               # without ln_scale: the statistics of out)
     ln_in_stats: torch.Tensor | None = None,   # f32 [rows, k/64, 2]: consumer mode
     ln_tab: torch.Tensor | None = None,        # f32 [4, >=n] rows c1_hi, c1_lo, c2_hi, c2_lo
     ln_rms: bool = False,                      # RMSNorm consumer: ln_in_stats without ln_tab, the norm's gain in w
@@ -81,7 +83,7 @@ def gemm(
         assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
     assert a.stride(-1) == 1 and w.stride(-1) == 1 and out.stride(-1) == 1
     m = a.shape[0]
-    g = _lib.GemmArgs()
+    g = _lib.GemmArgsDilated()
     g.a, g.lda = a.data_ptr(), a.stride(0)
     g.w, g.ldw = w.data_ptr(), w.stride(0)
     g.m = m
@@ -90,7 +92,7 @@ def gemm(
     g.rows_per_batch = rows_per_batch
     g.num_batches = num_batches
     g.batched_tiles = int(batched_tiles)
-    g.conv_taps, g.conv_pad, g.conv_grouped = conv_taps, conv_pad, int(conv_grouped)
+    g.conv_taps, g.conv_pad, g.conv_grouped, g.conv_dilation = conv_taps, conv_pad, int(conv_grouped), conv_dilation
     g.act = act
     g.out_bf16 = int(out.dtype == torch.bfloat16 or out_fp8)
     g.out_fp8 = int(out_fp8)
@@ -120,8 +122,11 @@ def gemm(
         assert out2.dtype == (torch.uint8 if out2_fp8 else torch.bfloat16) and out2.stride(-1) == 1
         g.out2_bf16, g.ldo2 = out2.data_ptr(), out2.stride(0)
     if ln_scale is not None:
-        assert ln_scale.dtype == torch.float32 and ln_stats is not None and ln_stats.dtype == torch.float32
-        g.ln_scale, g.ln_stats = ln_scale.data_ptr(), ln_stats.data_ptr()
+        assert ln_scale.dtype == torch.float32 and ln_stats is not None
+        g.ln_scale = ln_scale.data_ptr()
+    if ln_stats is not None:
+        assert ln_stats.dtype == torch.float32 and out2 is not None
+        g.ln_stats = ln_stats.data_ptr()
     if ln_rms:
         assert ln_in_stats is not None and ln_in_stats.dtype == torch.float32 and ln_tab is None
         g.ln_rms, g.ln_in_stats = 1, ln_in_stats.data_ptr()
@@ -140,5 +145,5 @@ def gemm(
     if out2_scale is not None:
         assert out2_scale.is_contiguous() and out2_scale.shape[-1] == m
         g.out2_scale = out2_scale.data_ptr()
-    _lib.check(_lib.load().f5_gemm_bf16(C.byref(g), _stream()))
+    _lib.check(_lib.load().f5_gemm_bf16(C.cast(C.pointer(g), C.POINTER(_lib.GemmArgs)), _stream()))
     return out

@@ -696,6 +696,16 @@ int f5_bigvgan_decode(const f5_bigvgan_weights* w, const f5_bigvgan_buffers* b, 
  * to device tables.  out: bf16 (out_bf16 = 1) or fp32, the same layout. */
 int f5_bigvgan_act_forward(const float* x, int32_t batch, int32_t rows_per_batch, int32_t channels,
                            const int32_t* lens, const f5_bigvgan_act* act, int32_t out_bf16, void* out, void* stream);
+/* Kernel test entry (ABI 2.007): the resblock mean out[i] = (xk[i] + xk[stride + i] + ... ) / nk over nk fp32 streams
+ * stride elements apart, i < n, summed in stream order in fp32 with one IEEE division; out bf16 (out_bf16 = 1) or fp32
+ * [n]. */
+int f5_bigvgan_resblock_mean(const float* xk, int64_t stride, int32_t nk, int64_t n, int32_t out_bf16, void* out,
+                             void* stream);
+/* Kernel test entry (ABI 2.007): conv_post, Conv1d(channels, 1, 7, padding=3) over x fp32 [batch, frames, channels]
+ * with zero padding inside each utterance, w fp32 [7, channels] tap-major, bias fp32 [1] or NULL, then tanh (use_tanh)
+ * or a clamp to [-1, 1]; out fp32 [batch, frames]. */
+int f5_bigvgan_conv_post(const float* x, int32_t batch, int32_t frames, int32_t channels, const float* w,
+                         const float* bias, int32_t use_tanh, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------ *
  * Host utilities for hosts that are not Python (the package's weights.PackedDiT / dit.DitSession / parallel.py do

@@ -257,7 +257,9 @@ def test_generate_cli_accepts_vocoder(monkeypatch):
 def test_abi_version_and_c_layout_of_new_structs(tmp_path):
     from f5_tts_mlx_b200 import _lib
     import f5_tts_mlx_b200.bigvgan as BV
-    assert _lib.load().f5_abi_version() >= 2005
+    assert _lib.load().f5_abi_version() >= 2007          # 2.007: the resblock-mean and conv_post test entries
+    for name in ("f5_bigvgan_resblock_mean", "f5_bigvgan_conv_post"):
+        assert hasattr(_lib.load(), name) and name in _lib.SYMBOLS
     assert C.sizeof(_lib.GemmArgsDilated) == C.sizeof(_lib.GemmArgs)
     gcc = shutil.which("gcc")
     if gcc is None:

@@ -5,7 +5,8 @@ utterances of the batch may change a single bit of it.
   b. bucket rows, at session level: a frame-bucketed session with the rows beyond frames_valid replaced;
   c. batch neighbours, at session level: utterance 1 replaced, utterances 0 and 2 compared;
   d. batch neighbours through sample() on one plan and its captured graph;
-  e. batch neighbours in the duration model and Vocos.
+  b-d again for the UNetT (E2TTS), whose rows are masked through seq_len1 / valid_len1 from the time row on;
+  e. batch neighbours in the duration model, Vocos and BigVGAN.
 
 Every comparison is bitwise.  Both runs of a comparison use the same plan, so shapes, tile choices and launches are
 identical; no kernel reduces across utterances, and the one atomic (the FP8 quantise pass's atomicMax of a tile's
@@ -111,8 +112,9 @@ def test_attention_masked_keys_cannot_reach_valid_rows(entry, N, poison):
 
 # ---------------------------------------------------------------- DiT sessions
 def drive(m, x, cond, text, tvals, ti, seq_len, n_valid):
-    """A CFG session of `m` with x and cond [B, frames, 100] as given on every row (frames > n_valid: a bucketed
-    session with frames_valid = n_valid): inputs, precompute, one forward.  Returns the stages [2, B, frames, C]."""
+    """A CFG session of `m` (a DiT or a UNetT) with x and cond [B, frames, 100] as given on every row (frames > n_valid:
+    a bucketed session with frames_valid = n_valid): inputs, precompute, one forward.  Returns the stages
+    [2, B, rows, C]: rows = frames, or frames + 1 for the UNetT's x and v (each utterance's time row first)."""
     B, NB = x.shape[:2]
     bucketed = NB != n_valid
     s = m.session(B, NB, tvals.numel(), True, text.shape[1], seq_len is not None, bucketed=bucketed)
@@ -126,7 +128,7 @@ def drive(m, x, cond, text, tvals, ti, seq_len, n_valid):
     m.precompute(s)
     m.forward_session(s, ti)
     torch.cuda.synchronize()
-    return s, {k: getattr(s, k).view(2, B, NB, -1).cpu() for k in STAGES}
+    return s, {k: (lambda t: t.view(2, B, t.shape[0] // (2 * B), -1))(getattr(s, k)).cpu() for k in STAGES}
 
 
 def bucket_text(text):
@@ -310,3 +312,117 @@ def test_vocos_neighbour_cannot_reach_utterance_0():
     b = voc.decode(mel2.to(DEV)).cpu()
     assert not torch.equal(a[1], b[1])
     assert_exact(b[:1], a[:1], lambda r, c: f"utterance 0 sample {c}", "vocos wave")
+
+
+@pytest.mark.parametrize("which", ["small", "released"])
+def test_bigvgan_neighbour_cannot_reach_other_utterances(which):
+    """B = 3: utterance 1's mel times 64, then with inf and NaN frames, leaves the waves of utterances 0 and 2 bitwise.
+    Every BigVGAN convolution runs batched tiles that never straddle utterances, with zero padding inside each one."""
+    from test_gpu_bigvgan import _vocoder
+    cfg, _, voc = _vocoder(which)
+    g = torch.Generator().manual_seed(63)
+    n = 20 if which == "small" else 8
+    mel = torch.randn(3, n, cfg.num_mels, generator=g) - 3.0
+    base = voc.decode(mel.to(DEV)).cpu()
+    for kind in ("x64", "nonfinite"):
+        mel2 = mel.clone()
+        if kind == "x64":
+            mel2[1] *= 64
+        else:
+            mel2[1, 2:4] = float("inf")
+            mel2[1, 5, ::3] = float("nan")
+            mel2[1, n - 1] = float("-inf")
+        got = voc.decode(mel2.to(DEV)).cpu()
+        assert not torch.equal(got[1], base[1]), f"{kind}: utterance 1 did not change"
+        for u in (0, 2):
+            assert_exact(got[u:u + 1], base[u:u + 1], lambda r, c, u=u: f"utterance {u} sample {c}",
+                         f"bigvgan {which} neighbour {kind}")
+
+
+# ---------------------------------------------------------------- b-d for the UNetT (E2TTS)
+UNETT_ROWS1 = ("x", "v")          # the stages with N + 1 rows per utterance (the time row first)
+
+
+def unett_model():
+    """A 4-layer, 256-wide UNetT with random weights (the E2TTS_Base structure: skips, RoPE on one head)."""
+    if "unett" not in _M:
+        from f5_tts_mlx_b200.unett import UNetT, UNetTConfig, random_unett_weights
+        cfg = UNetTConfig(dim=256, depth=4, heads=4, ff_mult=4)
+        _M["unett"] = UNetT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, ff_mult=cfg.ff_mult,
+                            text_num_embeds=cfg.text_num_embeds, text_dim=cfg.text_dim, pe_attn_head=cfg.pe_attn_head,
+                            device=DEV).load_weights(random_unett_weights(cfg, seed=71))
+    return _M["unett"]
+
+
+def test_unett_bucket_rows_cannot_reach_valid_rows():
+    """The UNetT in a bucketed session (256 frames, frames_valid 150, B = 2 with ragged seq_len, CFG): the bucket rows
+    of y_bf16 and of the padded cond hold zeros, +-1e4, then inf and NaN; both branches keep every bit of the first 150
+    rows of text_x, hoist and h and the first 151 rows (the time row and the 150 frames) of x and v."""
+    B, N, NB = 2, 150, 256
+    x, cond, text = inputs(B, N, 50, seed=81)
+    text = bucket_text(text)
+    seq_len = torch.tensor([150, 123], dtype=torch.int32)
+    tvals = eval_times("rk4")
+    m = unett_model()
+    g = torch.Generator().manual_seed(82)
+    runs = {}
+    for kind in ("zeros", "1e4", "nonfinite"):
+        xf = torch.cat([x, fill(kind, (B, NB - N, 100), g)], 1)
+        cf = torch.cat([cond, fill(kind, (B, NB - N, 100), g)], 1)
+        runs[kind] = drive(m, xf, cf, text, tvals, 2, seq_len, N)[1]
+    for kind in ("1e4", "nonfinite"):
+        for k in STAGES:
+            n = N + 1 if k in UNETT_ROWS1 else N
+            assert_rows_exact(runs[kind][k], runs["zeros"][k], [n] * B, range(B), f"unett bucket rows {kind}: {k}")
+
+
+@pytest.mark.parametrize("bucket", [False, True], ids=["exact", "bucket256"])
+def test_unett_batch_neighbour_cannot_reach_other_utterances(bucket):
+    """The UNetT at B = 3, N = 150 (exact, or a 256-frame bucket), CFG, ragged seq_len: with utterance 1 replaced
+    (NEIGHBOURS), every row of utterances 0 and 2 (their time row, padding and bucket rows included) keeps its bits in
+    text_x, hoist, h, x and v, in both branches."""
+    B, N = 3, 150
+    NB = 256 if bucket else N
+    x, cond, text = inputs(B, N, 50, seed=91)
+    if bucket:
+        text = bucket_text(text)
+    seq_len = torch.tensor([150, 131, 97], dtype=torch.int32)
+    tvals = eval_times("rk4")
+    m = unett_model()
+    pad = lambda a: F.pad(a, (0, 0, 0, NB - N))
+    g = torch.Generator().manual_seed(92)
+    base = drive(m, pad(x), pad(cond), text, tvals, 2, seq_len, N)[1]
+    for kind in NEIGHBOURS:
+        x2, c2, t2, s2 = neighbour(kind, x, cond, text, seq_len, g)
+        got = drive(m, pad(x2), pad(c2), t2, tvals, 2, s2, N)[1]
+        assert not torch.equal(got["v"][:, 1], base["v"][:, 1]), f"{kind}: utterance 1 did not change"
+        for k in STAGES:
+            n = NB + 1 if k in UNETT_ROWS1 else NB
+            assert_rows_exact(got[k], base[k], [n] * B, (0, 2),
+                              f"unett {'bucket' if bucket else 'exact'} neighbour {kind}: {k}")
+
+
+@pytest.mark.parametrize("bucket", [0, 128], ids=["exact", "bucket128"])
+@pytest.mark.parametrize("method", ["euler", "rk4"])
+def test_unett_sample_neighbours_cannot_reach_utterance_0(method, bucket):
+    """Two UNetT sample() calls (B = 3, CFG, 4 steps) on one plan, the second replaying the first's captured graph:
+    the neighbours' text, duration, cond and y0 change, utterance 0 keeps the bits of its out and whole trajectory."""
+    from f5_tts_mlx_b200 import F5TTS
+    B, N = 3, 150
+    f5 = F5TTS(unett_model())
+    kw = dict(steps=4, method=method, cfg_strength=2.0, sway_sampling_coef=-1.0, frame_bucket=bucket)
+    dur1, dur2 = torch.tensor([N, 131, 97]), torch.tensor([N, 101, 140])
+    cond1, text1, y01 = sample_call(B, N, 51, dur1)
+    cond2, text2, y02 = sample_call(B, N, 52, dur2)
+    cond2[0], text2[0], y02[0] = cond1[0], text1[0], y01[0]
+    out1, traj1 = f5.sample(cond1.to(DEV), text1, dur1, y0=y01, **kw)
+    plan, graph = f5.last_plan, f5.last_plan.graph
+    assert graph is not None
+    out2, traj2 = f5.sample(cond2.to(DEV), text2, dur2, y0=y02, **kw)
+    assert f5.last_plan is plan and plan.graph is graph, "the second call did not replay the first call's graph"
+    assert not torch.equal(out2[1], out1[1])
+    what = f"unett sample {method} {'bucket' if bucket else 'exact'}"
+    loc = lambda r, c: f"utterance 0 frame {r} column {c}"
+    assert_exact(out2[0].cpu(), out1[0].cpu(), loc, what + ": out")
+    for i in range(traj1.shape[0]):
+        assert_exact(traj2[i, 0].cpu(), traj1[i, 0].cpu(), loc, what + f": trajectory[{i}]")

@@ -18,7 +18,7 @@ import torch
 import torch.nn.functional as F
 
 from kernel_check import (E4M3_SUB, U32, U_E4M3, Guarded, act_bound, act_ref, assert_exact, assert_within, attn_tiles,
-                          cdiv, gemm_tile_count, gemm_tiles, instantiation, out_bound, round_to, rope_ref)
+                          bits, cdiv, gemm_tile_count, gemm_tiles, instantiation, out_bound, round_to, rope_ref)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -63,6 +63,24 @@ def pow2_scales(shape, seed, lo, hi):
     return torch.exp2(torch.randint(lo, hi + 1, shape, generator=g, device=DEV).float())
 
 
+def rms_row_stats(M, units, seed, zero_rows=()):
+    """RMSNorm consumer input: per row (sum, sum of squares) of every 64-column unit with the unit's sum of squares
+    64 4^e, e in {0, 1, 2, 3} per row, so the kernel's rsqrt(sum x^2 / (64 units)) = 2^-e exactly (rsqrtf is exact at
+    powers of two, as the fused-LN consumer cases rely on; 1 / (64 units) is exact for units a power of two).  The sums
+    are arbitrary integers (the RMS consumer must not read them).  zero_rows get all-zero statistics (their A rows are
+    zero too): the kernel clamps the sum to 1e-24, and 0 times its finite rstd is 0, so the output is the bias."""
+    assert units & (units - 1) == 0, "the RMS consumer is exact only for K / 64 a power of two"
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    e = torch.randint(0, 4, (M,), generator=g, device=DEV)
+    stats = torch.empty(M, units, 2, device=DEV)
+    stats[..., 0] = torch.randint(-50, 51, (M, units), generator=g, device=DEV).float()
+    stats[..., 1] = (64.0 * torch.exp2(2.0 * e.float()))[:, None]
+    rstd = torch.exp2(-e.double())
+    zr = torch.as_tensor(list(zero_rows), dtype=torch.long, device=DEV)
+    stats[zr] = 0.0
+    return stats, rstd
+
+
 def ln_row_stats(M, units, seed):
     """Fused-LN consumer input: per row (sum, sum of squares) of every 64-column unit such that mean and rstd are powers
     of two (mean 2, variance 2^20: rstd 2^-10; mean -4, variance 2^16: rstd 2^-8; the LayerNorm's 1e-6 is below half an
@@ -91,13 +109,18 @@ def assert_fp32_exact(x, what):
     assert torch.equal(x.float().double(), x), f"{what}: the float64 reference is not exact in fp32 (operands too large)"
 
 
-def conv_ref(A, W, *, M, N, K, rpb, nb, taps, pad, grouped):
+def conv_ref(A, W, *, M, N, K, rpb, nb, taps, pad, grouped, dilation=1):
     """float64 Conv1d of the implicit-GEMM operands: A [nb rpb, channels] (channels = N grouped, else K), W [N, taps K]
-    with W[n, t K + c] the weight of input channel c (of the column's 64-channel group when grouped) at tap t."""
-    cin = N if grouped else K
-    x = A.view(nb, rpb, cin).transpose(1, 2)
-    wt = W.view(N, taps, K).permute(0, 2, 1)
-    y = F.conv1d(x, wt, padding=pad, groups=N // 64 if grouped else 1)
+    with W[n, t K + c] the weight of input channel c (of the column's 64-channel group when grouped) at tap t; tap t of
+    frame m reads frame m + t dilation - pad."""
+    if not grouped:   # frames gathered per tap, one float64 matmul (cuBLAS) over [M, taps K]
+        src = torch.arange(rpb, device=A.device)[:, None] + torch.arange(taps, device=A.device)[None] * dilation - pad
+        ok = (src >= 0) & (src < rpb)
+        x = A.reshape(nb, rpb, K)[:, src.clamp(0, rpb - 1)] * ok[None, :, :, None]      # nb, rpb, taps, K
+        return x.reshape(M, taps * K) @ W.reshape(N, taps * K).T
+    x = A.reshape(nb, rpb, N).transpose(1, 2)
+    wt = W.reshape(N, taps, K).permute(0, 2, 1)
+    y = F.conv1d(x, wt, padding=pad, dilation=dilation, groups=N // 64)
     return y.transpose(1, 2).reshape(M, N)
 
 
@@ -108,7 +131,8 @@ def _sm_count():
 def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.0, rpb=0, nb=1, batched=False,
               row_len=False, gate=None, resid=None, out2=None, ln_scale=False, rope=False, ab8=False, pad_cols=0,
               act=0, scaled=False, out_blocks=False, scale_exp=(-3, 3), a_scale_ld=0, ln_in=False, conv_taps=1,
-              conv_pad=0, conv_grouped=False):
+              conv_pad=0, conv_grouped=False, conv_dilation=1, ln_rms=False, ln_stats=False, a_slot=False,
+              out2_slot=None, bias=True, rope_cols=0, rope_col2=0, q_cols=0):
     """One GEMM launch against its float64 reference.  out: 'bf16' | 'f32' | 'e4m3'; gate: None | 'shared' (one [N]
     vector for every utterance); resid: None | 'alias' (resid is out itself) | 'sep'; out2: None | 'bf16' | 'e4m3'.
 
@@ -118,7 +142,15 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
     scales must equal weights.quantize_e4m3_blocks of the float64 result bitwise.  out_blocks: block-scaled e4m3
     outputs of bf16 operands (the Mish producer of the block-scaled mode).
     ln_in: fused-LN consumer with power-of-two row statistics (ln_row_stats) and an integer c1 / c2 table.
-    conv_taps / conv_pad / conv_grouped: implicit Conv1d over batched utterances (conv_ref); K is the k per tap.
+    conv_taps / conv_pad / conv_grouped / conv_dilation: implicit Conv1d over batched utterances (conv_ref); K is the
+    k per tap.  W is [N, taps k_pad] with k_pad = K rounded up to 64 (BigVGAN's C = 96, 48, 24); its padding columns
+    hold nonzero integers that the reference ignores, so a k-block that reads past channel K of its row (the next
+    frame's channels instead of the TMA's zero fill) changes the result.
+    ln_rms: the RMSNorm consumer (UNetT) with power-of-two row scales (rms_row_stats) and all-zero rows 5 and M - 1.
+    ln_stats without ln_scale: the UNetT producer, out2 a plain bf16 copy of the fp32 out, ln_stats of it.
+    a_slot: A is the right half of a [M, 2K] buffer whose left half holds other integers (lda = 2K, a UNetT skip slot);
+    out2_slot 'left' | 'right': out2 is that half of a [M, 2N] buffer (ldo2 = 2N); the other half must stay untouched.
+    rope_cols / rope_col2 / q_cols (with rope): the rotated column ranges and the q_scale range; default 2N/3 and N/3.
     act (1 GELU-tanh, 2 GELU-erf, 3 Mish): the pre-activation is exact; the output must be (a) within act_bound of the
     float64 activation and (b) bitwise equal to the same GEMM launched in slices of at most SMs tiles, in which every tile
     is the first and only tile of its CTA."""
@@ -130,16 +162,28 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
     conv = conv_taps > 1 or conv_grouped
     assert not (conv and ab8) and (not conv or (rpb and batched)), "conv mode: bf16 operands, batched utterances"
     kin = N if conv_grouped else K
+    kp = -(-K // 64) * 64 if conv and not conv_grouped else K
     if ab8:
         A, W = ints((M, K), 2, seed, density, F8), ints((N, K), 2, seed + 1, density, F8)
         acc_scale = 1.0 if scaled else 0.5
     else:
-        A, W = ints((M, kin), amax, seed, density), ints((N, conv_taps * K), amax, seed + 1, density)
+        A, W = ints((M, kin), amax, seed, density), ints((N, conv_taps * kp), amax, seed + 1, density)
         acc_scale = 1.0
-    bias = ints((N,), 8, seed + 2, dtype=torch.float32)
+    if kp != K:       # the padding columns of every tap: nonzero, ignored by the reference
+        W.view(N, conv_taps, kp)[:, :, K:] = ints((N, conv_taps, kp - K), amax, seed + 11).abs() + 1
+    if a_slot:
+        slot = ints((M, 2 * K), amax, seed + 12)
+        slot[:, K:] = A
+        A = slot[:, K:]
+    zero_rows = (5, M - 1) if ln_rms else ()
+    if zero_rows:
+        A[list(zero_rows)] = 0
+    bias = ints((N,), 8, seed + 2, dtype=torch.float32) if bias else None
     rows = torch.arange(M, device=DEV)
     bidx, pos = rows // rpb_e, rows % rpb_e
-    A64, W64 = A.float().double(), W.float().double()
+    A64 = A.float().double()
+    W64 = W.float().double().view(N, conv_taps, kp)[:, :, :K].reshape(N, conv_taps * K) if kp != K else W.float().double()
+    bias64 = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device=DEV)
     kw = dict(bias=bias, tile_n=tile, w_static=bool(w_static), ab_fp8=ab8, acc_scale=acc_scale)
     colscale = torch.full((N,), acc_scale, dtype=torch.float64, device=DEV)
     sa_buf = None
@@ -154,25 +198,32 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
         colscale = sw.double()
         kw.update(a_scale=sa_buf, w_scale=sw)
     if conv:
-        cw = dict(M=M, N=N, K=K, rpb=rpb, nb=nb, taps=conv_taps, pad=conv_pad, grouped=conv_grouped)
+        cw = dict(M=M, N=N, K=K, rpb=rpb, nb=nb, taps=conv_taps, pad=conv_pad, grouped=conv_grouped,
+                  dilation=conv_dilation)
         acc, accb = conv_ref(A64, W64, **cw), conv_ref(A64.abs(), W64.abs(), **cw)
-        kw.update(n=N, k=K, conv_taps=conv_taps, conv_pad=conv_pad, conv_grouped=conv_grouped)
+        kw.update(n=N, k=K, conv_taps=conv_taps, conv_pad=conv_pad, conv_grouped=conv_grouped,
+                  conv_dilation=conv_dilation)
     else:
         acc, accb = A64 @ W64.T, A64.abs() @ W64.abs().T
     assert (accb < EXACT_LIMIT).all(), "operands too large for an exact test"     # bounds every partial sum
     stats = None
-    if ln_in:
+    if ln_rms:
+        stats, rstd = rms_row_stats(M, K // 64, seed + 9, zero_rows)
+        v = rstd[:, None] * acc + bias64[None]
+        vb = rstd[:, None] * accb + bias64.abs()[None]
+        kw.update(ln_rms=True, ln_in_stats=stats)
+    elif ln_in:
         stats, mean, rstd = ln_row_stats(M, K // 64, seed + 9)
         tab = ints((4, N + 8), 8, seed + 10, dtype=torch.float32)            # ld > N
         c1 = (tab[0] + tab[1])[:N].double()
-        c2 = (tab[2] + tab[3])[:N].double() + bias.double()
+        c2 = (tab[2] + tab[3])[:N].double() + bias64
         mu_r = (mean * rstd)[:, None]
         v = rstd[:, None] * colscale[None] * acc - mu_r * c1[None] + c2[None]
         vb = rstd[:, None] * colscale[None] * accb + (mu_r * c1[None]).abs() + c2.abs()[None]
         kw.update(ln_in_stats=stats, ln_tab=tab)
     else:
-        v = acc * colscale[None] + bias.double()
-        vb = accb * colscale[None] + bias.double().abs()
+        v = acc * colscale[None] + bias64
+        vb = accb * colscale[None] + bias64.abs()
     assert_fp32_exact(v, "pre-activation")
     bnd = None                                     # None: v is exact; else |kernel - v| <= bnd before the output rounding
     if act:
@@ -185,10 +236,12 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
         kw.update(rows_per_batch=rpb, num_batches=nb, batched_tiles=batched)
     if rope:
         tab_r = quarter_turns(rpb_e, seed + 3)
-        rc, qc = 2 * N // 3, N // 3
+        rc, qc = rope_cols or 2 * N // 3, q_cols or N // 3
         v = rope_ref(v, tab_r, pos, rc)
+        if rope_col2:
+            v[:, rope_col2:] = rope_ref(v[:, rope_col2:], tab_r, pos, rc)
         v[:, :qc] *= 0.125
-        kw.update(rope=tab_r, rope_cols=rc, q_scale=0.125, q_cols=qc)
+        kw.update(rope=tab_r, rope_cols=rc, rope_col2=rope_col2, q_scale=0.125, q_cols=qc)
     valid = torch.ones(M, dtype=torch.bool, device=DEV)
     lens = None
     if row_len:
@@ -227,20 +280,24 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
         so = Guarded(N // 64, M, torch.float32, DEV, lr=False)
         kw.update(out_scale=so.view)
     if out2 is not None:
-        g2 = Guarded(M, N, torch.uint8 if out2 == "e4m3" else torch.bfloat16, DEV)
-        kw.update(out2=g2.view, out2_fp8=out2 == "e4m3")
+        g2 = Guarded(M, 2 * N if out2_slot else N, torch.uint8 if out2 == "e4m3" else torch.bfloat16, DEV)
+        o2 = {None: slice(0, N), "left": slice(0, N), "right": slice(N, 2 * N)}[out2_slot]
+        other = slice(N, 2 * N) if out2_slot == "left" else slice(0, N)
+        kw.update(out2=g2.view[:, o2], out2_fp8=out2 == "e4m3")
         if blk_out2:
             s2 = Guarded(N // 64, M, torch.float32, DEV, lr=False)
             kw.update(out2_scale=s2.view)
-        if ln_scale:
-            s = pow2((N,), seed + 6).abs() - 1          # 1 + s in {0.5, 1, 2}
+        if ln_scale or ln_stats:
             st = Guarded(M, N // 64 * 2, torch.float32, DEV, lr=False)
-            kw.update(ln_scale=s, ln_stats=st.view.view(M, N // 64, 2))
-            want2 = v * (1 + s.double())
+            kw.update(ln_stats=st.view.view(M, N // 64, 2))
             if bnd is None:   # every partial unit sum (of squares) is a multiple of gq (gq^2) below 2^24 of them
                 gq = granularity(v)
                 u = v.view(M, N // 64, 64) / gq
                 assert (u.abs().sum(-1) < 2 ** 24).all() and ((u * u).sum(-1) < 2 ** 24).all(), "ln_stats would not be exact"
+        if ln_scale:
+            s = pow2((N,), seed + 6).abs() - 1          # 1 + s in {0.5, 1, 2}
+            kw.update(ln_scale=s)
+            want2 = v * (1 + s.double())
         else:
             want2 = v
         if out2 == "e4m3" and not blk_out2:
@@ -259,14 +316,19 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
     g_out.check(what + " out guard")
     if g2 is not None:
         sc = (1 + s.double()) if s is not None else torch.ones(N, dtype=torch.float64, device=DEV)
+        v2 = g2.view[:, o2]
         if blk_out2:
             # the scale rule of the float64 result (exact), or of the kernel's own fp32 out when that is not exact
             _check_blocks(g2, s2, want2 if bnd is None else g_out.view.double() * sc, None, loc, what + " out2")
         elif bnd is None:
-            assert_exact(g2.view, round_to(want2, g2.view.dtype), loc, what + " out2")
+            assert_exact(v2, round_to(want2, v2.dtype), loc, what + " out2")
         else:
-            assert_within(g2.view, want2, out_bound(want2, sc.abs() * bnd + U32 * want2.abs(), g2.view.dtype) + 1e-300,
+            assert_within(v2, want2, out_bound(want2, sc.abs() * bnd + U32 * want2.abs(), v2.dtype) + 1e-300,
                           loc, what + " out2")
+        if out2_slot:   # the slot's other half is not touched; then it counts as written for the guard check
+            half = g2.view[:, other]
+            assert (bits(half).long() & 0xFFFF == g2.pat).all(), f"{what} out2: the other half of the slot was written"
+            half.zero_()
         g2.check(what + " out2 guard")
     if st is not None:
         u = v.view(M, N // 64, 64)
@@ -281,7 +343,8 @@ def run_exact(*, M, N, K, tile, w_static, out="bf16", seed=0, amax=4, density=1.
                           what + " ln_stats")
         st.check(what + " ln_stats guard")
     if act:
-        _check_slices(ops, A, W, kw, g_out, g2, st, so, s2, r if resid == "alias" else None,
+        _check_slices(ops, A, W, kw, g_out, g2.view[:, o2] if g2 is not None else None, st, so, s2,
+                      r if resid == "alias" else None,
                       dict(M=M, N=N, tile=64 if conv_grouped else tile, rpb=rpb, nb=nb, batched=batched, lens=lens,
                            stats=stats, sa_buf=sa_buf, resid_sep=r if resid == "sep" else None), loc, what)
 
@@ -331,7 +394,7 @@ def _check_slices(ops, A, W, kw, g_out, g2, st, so, s2, r_alias, geo, loc, what)
     out_s = torch.empty(g_out.view.shape, dtype=g_out.view.dtype, device=DEV)
     if r_alias is not None:
         out_s.copy_(r_alias)
-    out2_s = torch.empty(g2.view.shape, dtype=g2.view.dtype, device=DEV) if g2 is not None else None
+    out2_s = torch.empty(g2.shape, dtype=g2.dtype, device=DEV) if g2 is not None else None
     st_s = torch.empty(st.view.shape, dtype=torch.float32, device=DEV) if st is not None else None
     so_s, s2_s = [], []
     for r0, r1, b0, b1 in cuts:
@@ -365,7 +428,7 @@ def _check_slices(ops, A, W, kw, g_out, g2, st, so, s2, r_alias, geo, loc, what)
     sl = what + f" vs {len(cuts)} one-wave slices"
     assert_exact(g_out.view, out_s, loc, sl + " out")
     if out2_s is not None:
-        assert_exact(g2.view, out2_s, loc, sl + " out2")
+        assert_exact(g2, out2_s, loc, sl + " out2")
     if st_s is not None:
         assert_exact(st.view, st_s, lambda r_, c_: f"row {r_} unit {c_ // 2}", sl + " ln_stats")
     if so is not None:
@@ -466,6 +529,91 @@ def test_gemm_exact_production(name, tile):
     run_exact(tile=tile, **PROD[name])
 
 
+# ---------------------------------------------------------------- UNetT (E2TTS_Base) launches, unett.cu
+# D 1024, F 4096, BU = 2 utterances of N1 = 938 rows (937 frames and the time row); the UNetT's row-wise GEMMs run
+# flat tiles, rows_per_batch only where RoPE positions or the row mask need it.  The skip slot of a layer is [R1, 2D]:
+# the pushed x (right half, also the QKV operand) beside the skip_proj operand (left half).
+_D, _FF, _N1 = 1024, 4096, 938
+UNETT = {
+    # QKV of RMSNorm(x): A the right half of a slot (lda 2D), RoPE on the leading head of q and of k, q scaled
+    "unett_qkv": dict(M=2 * _N1, N=3 * _D, K=_D, w_static=1, rpb=_N1, nb=2, a_slot=True, ln_rms=True, rope=True,
+                      rope_cols=64, rope_col2=_D, q_cols=_D, amax=2),
+    # QKV of a second-half layer: A is skip_proj's bf16 output (lda = D)
+    "unett_qkv_after_skip": dict(M=2 * _N1, N=3 * _D, K=_D, w_static=1, rpb=_N1, nb=2, ln_rms=True, rope=True,
+                                 rope_cols=64, rope_col2=_D, q_cols=_D, amax=2, seed=1),
+    # out-projection: x updated in place, rows beyond seq_len1 masked, bf16 copy + statistics without ln_scale
+    "unett_out_proj": dict(M=2 * _N1, N=_D, K=_D, w_static=1, rpb=_N1, nb=2, row_len=True, resid="alias", out="f32",
+                           out2="bf16", ln_stats=True, amax=1, density=0.125),
+    # the same without seq_len1 (one utterance, or a batch without padding): no row mask
+    "unett_out_proj_unmasked": dict(M=2 * _N1, N=_D, K=_D, w_static=1, rpb=_N1, nb=2, resid="alias", out="f32",
+                                    out2="bf16", ln_stats=True, amax=1, density=0.125, seed=3),
+    # FF1 of RMSNorm(x) with GELU-tanh
+    "unett_ff1": dict(M=2 * _N1, N=_FF, K=_D, w_static=1, ln_rms=True, act=1, amax=2),
+    # FF2 of a first-half layer: x in place, its bf16 copy pushed into the right half of the next slot with statistics
+    "unett_ff2_push": dict(M=2 * _N1, N=_D, K=_FF, w_static=1, resid="alias", out="f32", out2="bf16", out2_slot="right",
+                           ln_stats=True, amax=1, density=0.125),
+    # FF2 of a second-half layer: the bf16 copy beside its skip (left half), no statistics (skip_proj comes first)
+    "unett_ff2_skip": dict(M=2 * _N1, N=_D, K=_FF, w_static=1, resid="alias", out="f32", out2="bf16", out2_slot="left",
+                           amax=1, density=0.125),
+    # FF2 of the last layer: the bf16 copy and statistics for norm_out (ldo2 = D)
+    "unett_ff2_last": dict(M=2 * _N1, N=_D, K=_FF, w_static=1, resid="alias", out="f32", out2="bf16", ln_stats=True,
+                           amax=1, density=0.125, seed=2),
+    # skip_proj([x | skip]): k = 2D over the whole slot, no bias, fp32 x + bf16 copy + statistics
+    "unett_skip_proj": dict(M=2 * _N1, N=_D, K=2 * _D, w_static=1, bias=False, out="f32", out2="bf16", ln_stats=True,
+                            amax=1, density=0.125),
+    # proj_out(RMSNorm(x)): the 100 mel columns in fp32
+    "unett_proj_out": dict(M=2 * _N1, N=100, K=_D, w_static=1, ln_rms=True, out="f32"),
+}
+
+
+@pytest.mark.parametrize("tile", [64, 128])
+@pytest.mark.parametrize("name", list(UNETT))
+def test_gemm_exact_unett(name, tile):
+    run_exact(tile=tile, **UNETT[name])
+
+
+# ---------------------------------------------------------------- BigVGAN launches, bigvgan.cu f5_bigvgan_decode
+# The released config (bigvgan_v2_24khz_100band_256x): C0 = 1536, upsampling (kernel, rate) (8, 4) twice then (4, 2)
+# four times, resblock kernels 3 / 7 / 11 with dilations 1 / 3 / 5.  Every convolution is an implicit conv over B = 3
+# batched utterances; T in BIGVGAN_T crosses the 128-row tile edges and sits below the taps' reach (k = 11, d = 5 reads
+# 25 frames each side; decode at 6 mel frames runs stage 0 at T = 24).
+BIGVGAN_T = (1, 2, 24, 127, 128, 129, 300)
+BIGVGAN_C = (768, 384, 192, 96, 48, 24)
+
+
+def _bigvgan_cases():
+    from f5_tts_mlx_b200.bigvgan import polyphase_taps
+    cases = {"conv_pre": dict(N=1536, K=128, conv_taps=7, conv_pad=3)}          # over the mel padded to 128, bf16 out
+    for cin, k, u in ((1536, 8, 4), (768, 8, 4), (384, 4, 2), (192, 4, 2), (96, 4, 2), (48, 4, 2)):
+        taps, pad = polyphase_taps(k, u)
+        cases[f"ups_c{cin}_k{k}_u{u}"] = dict(N=u * (cin // 2), K=cin, conv_taps=taps, conv_pad=pad, out="f32")
+    for c in BIGVGAN_C:
+        for k in (3, 7, 11):
+            for d in (1, 3, 5):
+                cases[f"conv1_c{c}_k{k}_d{d}"] = dict(N=c, K=c, conv_taps=k, conv_pad=(k * d - d) // 2, conv_dilation=d,
+                                                      out="f32")
+            for r in ("sep", "alias"):   # conv2: the stage input as residual (m = 0), then the stream in place
+                cases[f"conv2_c{c}_k{k}_{r}"] = dict(N=c, K=c, conv_taps=k, conv_pad=(k - 1) // 2, out="f32", resid=r)
+    return cases
+
+
+BIGVGAN = _bigvgan_cases()
+
+
+@pytest.mark.parametrize("tile", [64, 128])
+@pytest.mark.parametrize("name", list(BIGVGAN))
+def test_gemm_exact_bigvgan(name, tile):
+    for T in BIGVGAN_T:
+        run_exact(M=3 * T, tile=tile, w_static=1, rpb=T, nb=3, batched=True, seed=T, **BIGVGAN[name])
+
+
+@pytest.mark.parametrize("tile", [64, 128])
+def test_gemm_exact_bigvgan_last_stage_waves(tile):
+    """The last stage's dilated conv (C = 24, k = 11, d = 5) over two utterances of 25 600 frames: 400 row tiles, so
+    every CTA of a 132-SM H100 walks at least three of them."""
+    run_exact(M=2 * 25600, tile=tile, w_static=1, rpb=25600, nb=2, batched=True, **BIGVGAN["conv1_c24_k11_d5"])
+
+
 def test_gemm_exact_modulation_table():
     """All AdaLN linears of every solver time as one GEMM: M = number of times, N = depth * 6 D + 2 D, 128 tiles."""
     run_exact(M=33, N=22 * 6 * 1024 + 2 * 1024, K=1024, tile=128, w_static=1, out="f32", amax=2)
@@ -549,7 +697,7 @@ def test_fp8_block_promotion_exact():
 
 def _declared():
     table = [inst_of(c) for c in GRID + EPI]
-    for c in PROD.values():
+    for c in list(PROD.values()) + list(UNETT.values()) + list(BIGVGAN.values()):
         table += [inst_of(dict(c, tile=t)) for t in (64, 128)]
     table += [inst_of(dict(out="f32", tile=128))]                              # modulation table
     table += [inst_of(dict(out="f32", tile=t)) for t in (64, 128)]             # conv7

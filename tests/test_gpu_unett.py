@@ -2,26 +2,23 @@
 
   * the GEMM epilogue's RMSNorm consumer mode (f5_gemm_args.ln_rms) against float64, all-zero rows included;
   * the time-token pack kernel, bitwise against torch;
-  * UNetT.__call__ and sample() against the test-side restatement (tests/unett_emul.py), within 3x the drift of its bf16
-    emulation, on a small config and at E2TTS_Base size; frame bucketing; a ragged batch; generate().
+  * UNetT.__call__ and sample() against the test-side restatement (tests/unett_emul.py), frame by frame
+    (composed_check.assert_rows: every frame within 3x the worst frame of its bf16 emulation, every utterance within the
+    per-utterance rel rule), on a small config and at E2TTS_Base size, at lengths whose N + 1 rows (the time row
+    first) end just before, on and after a 128-row tile edge; frame bucketing; a ragged batch; generate().
 """
 import ctypes as C
 
 import pytest
 import torch
 
+from composed_check import assert_rows
 from helpers import rel, synth_audio
 from oracle import f5_oracle as O
 import unett_emul as U
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def within_drift(got, ref, ref16, factor=3.0, floor=2e-3):
-    drift, r = rel(ref16, ref), rel(got, ref)
-    assert torch.isfinite(got).all() and r < max(factor * drift, floor), f"rel {r:.3e} vs bf16 drift {drift:.3e}"
-    return r, drift
 
 
 # ---------------------------------------------------------------- kernels
@@ -135,21 +132,35 @@ def test_forward_vs_restatement(which, drops, request):
     ref = U.unett_forward(x, cond, text, t, *drops, None, W, cfg)
     ref16 = U.unett_forward(x, cond, text, t, *drops, None, W, cfg, O.Precision(True))
     got = net(x.to(DEV), cond.to(DEV), text.to(DEV), t, *drops).cpu()
-    r, drift = within_drift(got, ref, ref16)
-    print(f"{which} drops={drops}: rel {r:.3e}, bf16 drift {drift:.3e}")
+    rep = assert_rows(got[None], ref[None], ref16[None], what=f"{which} drops={drops}")
+    print(f"{which} drops={drops}: {rep}")
 
 
-@pytest.mark.parametrize("which", ["small", "base"])
-def test_forward_ragged_batch_vs_restatement(which, request):
+def _forward_ragged(which, N, lens, request):
+    """B = 2 with a row mask (seq_len), frame by frame over each utterance's valid frames."""
     cfg, W, net = request.getfixturevalue(which)
-    x, cond, text = _inputs(2, 150, 40, seed=9, pad_from=31)
-    mask = torch.arange(150)[None] < torch.tensor([150, 97])[:, None]
+    x, cond, text = _inputs(2, N, 40, seed=9 + N, pad_from=31)
+    mask = torch.arange(N)[None] < torch.tensor(lens)[:, None]
     t = torch.tensor(0.61)
     ref = U.unett_forward(x, cond, text, t, False, False, mask, W, cfg)
     ref16 = U.unett_forward(x, cond, text, t, False, False, mask, W, cfg, O.Precision(True))
     got = net(x.to(DEV), cond.to(DEV), text.to(DEV), t, mask=mask.to(DEV)).cpu()
-    r, drift = within_drift(got[mask], ref[mask], ref16[mask])
-    print(f"{which} ragged: rel {r:.3e}, bf16 drift {drift:.3e}")
+    rep = assert_rows(got[None], ref[None], ref16[None], lens=lens, what=f"{which} ragged N={N} lens={lens}")
+    print(f"{which} ragged N={N}: {rep}")
+
+
+@pytest.mark.parametrize("which", ["small", "base"])
+def test_forward_ragged_batch_vs_restatement(which, request):
+    _forward_ragged(which, 150, (150, 97), request)
+
+
+@pytest.mark.parametrize("which", ["small", "base"])
+@pytest.mark.parametrize("N,lens", [(127, (127, 64)), (128, (128, 127)), (200, (200, 127))])
+def test_forward_tile_edges_vs_restatement(which, N, lens, request):
+    """The UNetT runs N + 1 rows per utterance (the time row first), so N = 127 / 128 / 200 put the last frame on, just
+    past and well past a 128-row tile edge, and the second utterance's rows start mid-tile: a frame lost or shifted at
+    the time row or at a tile edge is one bad row, which the per-frame check names."""
+    _forward_ragged(which, N, lens, request)
 
 
 @pytest.mark.parametrize("method", ["euler", "midpoint"])
@@ -165,8 +176,8 @@ def test_sample_cfg_vs_restatement(method, small):
     out, _ = F5TTS(net).sample(cond.to(DEV), text, N, **kw)
     ref, _ = U.sample(cond, text, N, W, cfg, **kw)
     ref16, _ = U.sample(cond, text, N, W, cfg, prec=O.Precision(True), **kw)
-    r, drift = within_drift(out.cpu(), ref, ref16)
-    print(f"{method} sample: rel {r:.3e}, bf16 drift {drift:.3e}")
+    rep = assert_rows(out.cpu()[None], ref[None], ref16[None], what=f"{method} sample")
+    print(f"{method} sample: {rep}")
 
 
 def test_sample_ragged_batch_vs_restatement(small):
@@ -180,8 +191,8 @@ def test_sample_ragged_batch_vs_restatement(small):
     out, _ = F5TTS(net).sample(cond.to(DEV), text, dur, **kw)
     ref, _ = U.sample(cond, text, dur, W, cfg, **kw)
     ref16, _ = U.sample(cond, text, dur, W, cfg, prec=O.Precision(True), **kw)
-    r, drift = within_drift(out.cpu(), ref, ref16)
-    print(f"ragged sample: rel {r:.3e}, bf16 drift {drift:.3e}")
+    rep = assert_rows(out.cpu()[None], ref[None], ref16[None], lens=dur.tolist(), what="ragged sample")
+    print(f"ragged sample: {rep}")
 
 
 def test_frame_bucketing_equals_exact_shapes(small):

@@ -164,6 +164,127 @@ def test_every_instantiation_has_gpu_cases_at_each_tile_width():
     assert not missing, f"instantiations without a GPU case: {missing}"
 
 
+def gemm_form(f: dict) -> tuple:
+    """The form of one f5_gemm_bf16 launch, from its nonzero fields (names of f5_gemm_args): which optional inputs and
+    outputs are set, the activation and output type, and how lda compares with k and ldo2 with n ('=' or '2x': half of
+    a slot twice as wide)."""
+    rel = lambda ld, x: "=" if ld == x else ("2x" if ld == 2 * x else ">")
+    return (("bias", "bias" in f),
+            ("resid", ("alias" if f["resid"] == f["out"] else "sep") if "resid" in f else None),
+            ("act", int(f.get("act", 0))), ("out_bf16", "out_bf16" in f),
+            ("rope", (int(f["rope_cols"]), int(f.get("rope_col2", 0)), int(f["q_cols"])) if "rope" in f else None),
+            ("ln_rms", "ln_rms" in f), ("ln_stats", "ln_stats" in f), ("row_len", "row_len" in f),
+            ("rows_per_batch", "rows_per_batch" in f), ("gate", "gate" in f), ("conv_taps", int(f.get("conv_taps", 1))),
+            ("lda", rel(int(f["lda"]), int(f["k"]))),
+            ("out2", rel(int(f["ldo2"]), int(f["n"])) if "out2_bf16" in f else None))
+
+
+def case_form(c: dict) -> tuple:
+    """gemm_form of a run_exact case (test_gpu_kernel_exact.UNETT): the fields unett.cu would set for it."""
+    f = {"k": c["K"], "n": c["N"], "lda": 2 * c["K"] if c.get("a_slot") else c["K"], "out": "x"}
+    if c.get("bias", True):
+        f["bias"] = 1
+    if c.get("resid"):
+        f["resid"] = "x" if c["resid"] == "alias" else "r"
+    if c.get("act"):
+        f["act"] = c["act"]
+    if c.get("out", "bf16") == "bf16":
+        f["out_bf16"] = 1
+    if c.get("rope"):
+        f.update(rope=1, rope_cols=c["rope_cols"], rope_col2=c.get("rope_col2", 0), q_cols=c["q_cols"])
+    for k in ("ln_rms", "ln_stats", "row_len", "gate"):
+        if c.get(k):
+            f[k] = 1
+    if c.get("rpb"):
+        f["rows_per_batch"] = c["rpb"]
+    if c.get("out2"):
+        f.update(out2_bf16=1, ldo2=2 * c["N"] if c.get("out2_slot") else c["N"])
+    return gemm_form(f)
+
+
+def _scale_dims(form: tuple, D: int) -> tuple:
+    """A form with the rope column counts in units of the model width (the trace runs a narrower model than E2TTS_Base)."""
+    d = dict(form)
+    if d["rope"] is not None:
+        rc, c2, qc = d["rope"]
+        d["rope"] = (rc, c2 / D, qc / D)
+    return tuple(d.items())
+
+
+def test_every_unett_gemm_form_has_a_known_answer_case():
+    """Every f5_gemm_bf16 launch of f5_unett_forward from the time token to proj_out (the UNetT's own launches; the input
+    embedding is the DiT's, tested as test_gpu_kernel_exact.PROD) in every traced mode is the form of one of the
+    declared UNETT cases.  A new UNetT launch form without a known-answer GPU case fails here."""
+    import sys
+    sys.path.insert(0, str(ROOT / "tests" / "golden"))
+    import make_launch_trace as T
+    import test_gpu_kernel_exact as ex
+    declared = {_scale_dims(case_form(c), 1024): name for name, c in ex.UNETT.items()}
+    seen = {}
+    for header, lines in T.cases(T.launch_trace()):
+        if not header.startswith("unett"):
+            continue
+        pack = re.search(r"launch_unett_time_pack\(.*\bD=(\d+)", "\n".join(lines))
+        if pack is None:         # a case that stops before the forward (precompute alone, a refusal)
+            continue
+        D = int(pack[1])
+        after = False
+        for line in lines:
+            if "launch_unett_time_pack(" in line:
+                after = True
+            elif after and line.startswith("  f5_gemm_bf16("):
+                f = dict(re.findall(r"(\w+)=([^,()]+)", line[line.index("(") + 1:]))
+                form = _scale_dims(gemm_form(f), D)
+                assert form in declared, f"{header}: a UNetT GEMM form without a known-answer case:\n{line}\n{form}"
+                seen[declared[form]] = True
+                after = f["out"] != "ub.v"          # proj_out into v ends the forward
+    assert set(seen) == set(ex.UNETT), f"declared UNETT cases the trace never launches: {set(ex.UNETT) - set(seen)}"
+
+
+# BigVGAN's host code (bigvgan.cu f5_bigvgan_decode) is not traced: its GEMM forms, listed from the source, and the
+# BIGVGAN cases of test_gpu_kernel_exact that launch each one.  (taps, dilation > 1, bf16 out, residual)
+BIGVGAN_FORMS = {
+    "conv_pre": (7, False, True, None),          # 7 taps over the mel padded to 128 columns, bf16 operand out
+    "ups": ("polyphase", False, False, None),    # polyphase transposed conv, fp32 out
+    "conv1": ("k", True, False, None),           # dilated conv, fp32 out
+    "conv2_m0": ("k", False, False, "sep"),      # conv2 of m = 0: the stage input as residual
+    "conv2_m12": ("k", False, False, "alias"),   # conv2 of m = 1, 2: resid == out, the stream updated in place
+}
+
+
+def test_bigvgan_gemm_forms_have_known_answer_cases():
+    import test_gpu_kernel_exact as ex
+    src = (ROOT / "f5_tts_mlx_b200" / "csrc" / "bigvgan.cu").read_text()
+    # the launches BIGVGAN_FORMS restates are still the ones decode makes.  The lines are matched verbatim, so a mere
+    # reformatting of f5_bigvgan_decode trips this too: then update the lines here after checking that the forms (taps,
+    # dilation, output type, residual) are unchanged, or add a case to BIGVGAN and BIGVGAN_FORMS if one is new.
+    for line in ("g.a = b->mel_bf16; g.lda = 128; g.w = w->conv_pre_w; g.ldw = 7 * 128;",
+                 "g.conv_taps = 7; g.conv_pad = 3;",
+                 "g.out_bf16 = 1; g.q_scale = 1.f;",
+                 "conv(b->a_bf16, T, C, w->up_w[i], w->up_taps[i], w->up_pad[i], 1, w->up_b[i], u * Co, b->x_up, false,",
+                 "conv(b->a_bf16, T, C, blk.conv1_w[m], k, (k * d - d) / 2, d, blk.conv1_b[m], C, b->t, false,",
+                 "conv(b->a_bf16, T, C, blk.conv2_w[m], k, (k - 1) / 2, 1, blk.conv2_b[m], C, xj, false, xin)",
+                 "xin = xj;"):
+        assert line in src, line
+    assert src.count("f5_gemm_bf16(&g, st)") == 2 and src.count("conv(b->a_bf16") == 3
+    forms = {"conv_pre": [], "ups": [], "conv1": [], "conv2_m0": [], "conv2_m12": []}
+    for name, c in ex.BIGVGAN.items():
+        if name == "conv_pre":
+            forms["conv_pre"].append(name)
+            assert c["conv_taps"] == 7 and c["conv_pad"] == 3 and c.get("out", "bf16") == "bf16" and c["K"] == 128
+        elif name.startswith("ups"):
+            forms["ups"].append(name)
+        elif name.startswith("conv1"):
+            forms["conv1"].append(name)
+        else:
+            forms["conv2_m0" if c["resid"] == "sep" else "conv2_m12"].append(name)
+    assert all(forms.values()), forms
+    released = {(c, k, d) for c in ex.BIGVGAN_C for k in (3, 7, 11) for d in (1, 3, 5)}
+    assert {(c["N"], c["conv_taps"], c.get("conv_dilation", 1)) for n, c in ex.BIGVGAN.items()
+            if n.startswith("conv1")} == released
+    assert set(BIGVGAN_FORMS) == set(forms)
+
+
 def test_launch_geometry_restates_the_launcher():
     """kernel_check's tile width and tile count follow f5_gemm_bf16 (gemm.cu) on known answers."""
     from kernel_check import gemm_bn, gemm_num_kb, gemm_tile_count
