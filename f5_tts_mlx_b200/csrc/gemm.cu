@@ -76,7 +76,19 @@ static int dispatch_scaled(int act, bool out_bf16, bool rope, const CUtensorMap&
                    "resid=%d", act, (int)out_bf16, (int)rope, (int)resid);
 }
 
+// Drain each CTA's last 128-wide tile on both consumer warpgroups (GemmParams::tail_split); only tests turn it off,
+// to compare against the single-warpgroup drain
+static int g_tail_split = 1;
+
 }  // namespace f5
+
+// Test hook, not part of include/f5_b200.h: sets whether later f5_gemm_bf16 launches split the last tile's drain (the
+// outputs are the same either way); returns the previous setting.
+extern "C" int f5_gemm_test_tail_split(int enable) {
+  const int prev = f5::g_tail_split;
+  f5::g_tail_split = enable != 0;
+  return prev;
+}
 
 extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   using namespace f5;
@@ -191,6 +203,7 @@ extern "C" int f5_gemm_bf16(const f5_gemm_args* a, void* stream_) {
   p.ab8 = ab8 ? 1 : 0; p.acc_scale = ab8 ? a->acc_scale : 1.f; p.out2_fp8 = a->out2_fp8; p.out_fp8 = a->out_fp8;
   p.a_scale = a->a_scale; p.a_scale_ld = a->a_scale_ld; p.w_scale = a->w_scale;
   p.out_scale = a->out_scale; p.out2_scale = a->out2_scale;
+  p.tail_split = g_tail_split;
   if (a->out2_bf16) F5_REQUIRE(a->ldo2 % 8 == 0 && a->n % 8 == 0, "f5_gemm_bf16: out2 alignment");
 
   // A: (channels, frames, utterances); flat mode is one "utterance" of m rows

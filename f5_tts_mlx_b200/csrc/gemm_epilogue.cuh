@@ -63,6 +63,9 @@ struct GemmParams {
   // RMSNorm consumer (f5_gemm_args.ln_rms): the row scale is sqrt(K) / max(||x||, 1e-12) from ln_in_stats, no mean
   // term and no ln_tab (the norm's gain is folded into W)
   int ln_rms;
+  // BN = 128, no RoPE: the CTA's last tile is drained by both consumer warpgroups, one 64-column unit each; 0
+  // drains it on its owner alone, bit for bit the same outputs (f5_gemm_test_tail_split)
+  int tail_split;
 };
 
 // Each CTA touches its 1/num_ctas slice of [pf_ptr, pf_ptr + pf_bytes) with L2 prefetches (one warp,
@@ -509,25 +512,26 @@ __device__ __forceinline__ void acc_ld32(const uint8_t* box, int r, uint32_t (&a
   }
 }
 
-// Drains one accumulator tile of BN columns (st.acc: its BN / 32 fp32 boxes; this thread's row st.r).  `res0` holds the
-// residual of the first 32 columns (loaded here instead in the RoPE and block-scaled forms).
+// Drains the 64-column units [cc0, cc0 + ncc) of an accumulator tile of BN columns (st.acc: its BN / 32 fp32 boxes;
+// this thread's row st.r).  `res0` holds the residual of unit cc0's first 32 columns (loaded here instead in the RoPE
+// and block-scaled forms).
 template <int BN, int ACT, bool OUT_BF16, bool ROPE, bool SC = false>
 __device__ __forceinline__ void epi_drain_tile(const float* bias_s, const float* gate_s, const float* aux_s,
                                                const float2 (&cs)[ROPE ? 32 : 1], float4 (&res0)[8], const GemmParams& p,
-                                               int n0, int row, bool row_ok, bool row_valid, const EpiStage& st,
-                                               const float* ws_s = nullptr) {
+                                               int n0, int cc0, int ncc, int row, bool row_ok, bool row_valid,
+                                               const EpiStage& st, const float* ws_s = nullptr) {
   float4 res1[8];
   float2 unit_acc = make_float2(0.f, 0.f);
   float unit_amax = 0.f;
 #pragma unroll 1
-  for (int cc = 0; cc < BN / 64; ++cc) {
+  for (int cc = cc0; cc < cc0 + ncc; ++cc) {
     const int colA = n0 + cc * 64, colB = colA + 32;
     uint32_t acc[32];
     // chunk A (first half of the head): request chunk B's residual, then drain A.  A later unit's first residual is
     // requested here too, not under the previous chunk B.  The RoPE and block-scaled epilogues hold more registers
     // (the head's cos / sin, the unit's amax): they request chunk B's residual after chunk A (RoPE GEMMs get none).
     constexpr bool kLateB = ROPE || SC;
-    if (kLateB || cc > 0) epi_load_resid(p, row, colA, row_ok, res0);
+    if (kLateB || cc > cc0) epi_load_resid(p, row, colA, row_ok, res0);
     if constexpr (!kLateB) epi_load_resid(p, row, colB, row_ok, res1);
     acc_ld32(st.acc + (2 * cc) * 16384, st.r, acc);
     if (colA < p.N)   // uniform per CTA
